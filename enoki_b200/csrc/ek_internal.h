@@ -59,8 +59,8 @@ struct EkContext {
     std::vector<uint32_t> free_handles;
     std::set<uint32_t> live;            /* jit.cu:166-167 */
     uint64_t next_seq = 1;              /* EkVariable::seq counter */
-    int fast_mode = 1;                  /* 32-bit fast sweep kernel: 1 = use it, 0 = general kernels only (set by ek_init:
-                                           EK_FAST / kernel qualification, see ek_qualify.cpp; ek_set_fast_mode) */
+    int fast_mode = 1;                  /* 32-bit fast sweep kernel: 1 = use it, 0 = general kernels only (ek_set_fast_mode;
+                                           ek_init() leaves it as it is) */
     std::vector<uint32_t> dirty;        /* jit.cu:169-170 */
     std::unordered_map<const void *, uint32_t> ptr_map;    /* jit.cu:178-179 */
     uint32_t scatter_gather_operand = 0;

@@ -15,13 +15,6 @@
 #include <sstream>
 #include <string>
 #include <vector>
-#include <dlfcn.h>
-#include <signal.h>
-#include <spawn.h>
-#include <sys/stat.h>
-#include <sys/wait.h>
-#include <unistd.h>
-extern char **environ;
 
 static EkContext *g_ctx = nullptr;
 static thread_local std::string g_error;
@@ -79,91 +72,6 @@ int ek_set_device(int ordinal) {
     return 0;
 }
 
-/* ---- kernel qualification ---------------------------------------------------------------------------------------
-   The 32-bit fast sweep kernel (ek_sweep_fast.cu) was written in round 2 after this repository had lost its access to
-   GPU hardware, so nothing in the tree has seen it run.  The runtime therefore does not trust it blindly: the first
-   ek_init() on a machine runs `ek_qualify` (enoki_b200/ek_qualify, built from csrc/ek_qualify.cpp) in a CHILD PROCESS.
-   The child evaluates a battery of programs twice -- through the general sweep kernels that passed the round-1 GPU
-   test-suite, and through the fast kernel -- and compares the results bit for bit.  Only when every comparison agrees
-   (exit status 0, within 150 s) is the fast kernel used; a wrong result, a CUDA error, a watchdog trap or a crash of the
-   child all leave this process on the general kernels, with one line on stderr.  The verdict is remembered in a stamp
-   file keyed on the library file and the GPU name, so the battery runs once per machine, not once per process.  The
-   stamp and the battery's timings live in the temporary directory ($TMPDIR, else /tmp), never next to the library:
-   the installed tree may be read-only and stays unchanged by use.
-   EK_FAST=0 / EK_FAST=1 skip the qualification and force the answer (the child itself runs with EK_FAST=0 and switches
-   modes through ek_set_fast_mode()). */
-static std::string lib_path() {
-    Dl_info info;
-    if (dladdr((const void *) &ek_init, &info) && info.dli_fname) return info.dli_fname;
-    return "";
-}
-static int decide_fast_mode(const char *gpu_name) {
-    if (const char *e = getenv("EK_FAST")) return atoi(e) != 0 ? 1 : 0;
-    const std::string lib = lib_path();
-    if (lib.empty()) return 0;
-    const std::string dir = lib.substr(0, lib.find_last_of('/'));
-    const std::string helper = dir + "/ek_qualify";
-    struct stat st_lib, st_helper;
-    if (stat(lib.c_str(), &st_lib) != 0) return 0;
-    if (stat(helper.c_str(), &st_helper) != 0) {
-        fprintf(stderr, "enoki_b200: %s not found -- the fast sweep kernel stays off (general kernels are used)\n", helper.c_str());
-        return 0;
-    }
-    char key[512];
-    snprintf(key, sizeof(key), "lib %lld %lld gpu %s", (long long) st_lib.st_size, (long long) st_lib.st_mtime, gpu_name);
-    const char *tmpdir = getenv("TMPDIR");
-    const std::string tmp = (tmpdir && *tmpdir) ? tmpdir : "/tmp";
-    const std::string uid = std::to_string((long) getuid());
-    std::string stamps[1] = { tmp + "/ek_b200_fast_qualified_" + uid };
-    for (const std::string &sp : stamps) {
-        FILE *f = fopen(sp.c_str(), "r");
-        if (!f) continue;
-        char line[600] = { 0 }; int verdict = -1;
-        if (fgets(line, sizeof(line), f)) { size_t l = strlen(line); while (l && (line[l - 1] == '\n' || line[l - 1] == '\r')) line[--l] = 0; }
-        if (fscanf(f, "%d", &verdict) != 1) verdict = -1;
-        fclose(f);
-        if (verdict >= 0 && strcmp(line, key) == 0) return verdict ? 1 : 0;
-    }
-    /* run the battery in a child process (this process may already hold CUDA state: no fork-without-exec) */
-    pid_t pid = 0;
-    const std::string timing_file = tmp + "/ek_b200_fast_timing_" + uid + ".json";
-    char *argv[] = { const_cast<char *>(helper.c_str()), const_cast<char *>(timing_file.c_str()), nullptr };
-    std::vector<std::string> envs;
-    for (char **e = environ; e && *e; ++e) if (strncmp(*e, "EK_FAST=", 8) != 0) envs.push_back(*e);
-    envs.push_back("EK_FAST=0");
-    std::vector<char *> envp;
-    for (auto &e : envs) envp.push_back(const_cast<char *>(e.c_str()));
-    envp.push_back(nullptr);
-    int verdict = 0;
-    if (posix_spawn(&pid, helper.c_str(), nullptr, nullptr, argv, envp.data()) != 0) {
-        fprintf(stderr, "enoki_b200: could not start %s -- the fast sweep kernel stays off\n", helper.c_str());
-    } else {
-        int status = 0; bool done = false;
-        for (int waited_ms = 0; waited_ms < 150000; waited_ms += 50) {
-            pid_t r = waitpid(pid, &status, WNOHANG);
-            if (r == pid) { done = true; break; }
-            if (r < 0) break;
-            usleep(50000);
-        }
-        if (!done) { kill(pid, SIGKILL); waitpid(pid, &status, 0); }
-        verdict = (done && WIFEXITED(status) && WEXITSTATUS(status) == 0) ? 1 : 0;
-        if (!verdict)
-            fprintf(stderr, "enoki_b200: the fast sweep kernel did NOT qualify on this machine (%s) -- general kernels are used\n",
-                    !done ? "timeout" : WIFSIGNALED(status) ? "child crashed" :
-                    (WIFEXITED(status) && WEXITSTATUS(status) == 4) ? "correct, but not faster than the general kernel here" : "results differ / CUDA error, see above");
-    }
-    for (const std::string &sp : stamps) {
-        const std::string tmp = sp + "." + std::to_string((long) getpid());
-        FILE *f = fopen(tmp.c_str(), "w");
-        if (!f) continue;
-        fprintf(f, "%s\n%d\n", key, verdict);
-        fclose(f);
-        if (rename(tmp.c_str(), sp.c_str()) == 0) break;
-        unlink(tmp.c_str());
-    }
-    return verdict;
-}
-
 int ek_init(void) {
     EkContext &ctx = ek_ctx();
     if (ctx.initialized) return 0;
@@ -192,7 +100,6 @@ int ek_init(void) {
     ek_cuda_check(cudaMalloc(&ctx.red_counters, sizeof(uint32_t) * EK_MAX_RED));
     ek_cuda_check(cudaMemset(ctx.red_counters, 0, sizeof(uint32_t) * EK_MAX_RED));
     ctx.initialized = true;
-    ctx.fast_mode = decide_fast_mode(prop.name);
     static bool registered = false;
     if (!registered) { atexit(ek_shutdown); registered = true; }   /* jit.cu:315-318 */
     return 0;

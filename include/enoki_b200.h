@@ -254,8 +254,8 @@ EK_API int  ek_allreduce(ek_type type, void *data, size_t count);    /* in-place
 EK_API int  ek_allreduce_scalars(const uint32_t *handles, size_t n); /* evaluate + sum the given variables over all ranks */
 EK_API void ek_dist_shutdown(void);
 
-/* 32-bit fast sweep kernel (no counterpart in the reference): ek_init() enables it after the kernel qualification
-   described in csrc/ek_runtime.cpp (or as EK_FAST=0/1 says); these calls read / override that decision. */
+/* 32-bit fast sweep kernel (no counterpart in the reference): on by default; these calls read / override that
+   (0 = general kernels only). */
 EK_API void ek_set_fast_mode(int enable);
 EK_API int  ek_fast_mode(void);
 EK_API void ek_stats_reset(void);

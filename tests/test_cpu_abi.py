@@ -262,15 +262,27 @@ def test_resize_of_a_lazy_reduction_broadcasts(ek):
     gc.collect(); ek.lib().ek_debug_discard_side_effects()
 
 
-def test_qualification_battery_records_and_plans():
-    """enoki_b200/ek_qualify --dry: every program of the kernel-qualification battery (csrc/ek_qualify.cpp) is recorded
-    through the C ABI and planned in both modes (general kernels / fast kernel) on the host -- the battery itself must not be
-    what fails on the GPU box."""
-    import os
-    import subprocess
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    exe = os.path.join(root, "enoki_b200", "ek_qualify")
-    assert os.path.exists(exe), "enoki_b200/ek_qualify is not built (make -C enoki_b200/csrc)"
-    r = subprocess.run([exe, "--dry"], capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0, r.stderr[-2000:]
-    assert "recorded and planned in both modes" in r.stderr
+def test_sweep_battery_records_and_plans(ek):
+    """Every program of the sweep-kernel A/B battery (tests/sweep_battery.py, evaluated by test_gpu_sweep_ab.py) is
+    recorded and planned with the fast kernel off and on, on the host over fake device addresses: the battery itself must
+    not be what fails on the GPU."""
+    import gc
+    import itertools
+    import sweep_battery
+    L = ek.lib()
+    gc.collect(); L.ek_debug_discard_side_effects(); gc.collect()
+    addresses = itertools.count(0x7f0000000000, 0x100000000)
+
+    def evaluate(var=None):
+        ek.debug_plan()
+        L.ek_debug_discard_side_effects()
+    names = []
+    try:
+        for fast in (0, 1):
+            L.ek_set_fast_mode(fast)
+            names.append([r.name for r in sweep_battery.battery(lambda cls, a: cls.map(next(addresses), len(a)), evaluate)])
+    finally:
+        L.ek_set_fast_mode(1)
+    assert names[0] == names[1]
+    assert len(names[0]) == 244
+    assert ek.debug_plan() == ""

@@ -77,7 +77,7 @@ def _differential(ek, oracle, table, outputs, float_tol=()):
 
 @pytest.mark.parametrize("n", [4097, 20_011])
 def test_directed_programs_numpy_vs_host_compiled_kernel(ek, oracle, P, n):
-    """The programs of the kernel-qualification battery (csrc/ek_qualify.cpp `directed`): mask outputs (8-bit stores)
+    """The programs of the sweep-kernel A/B battery (tests/sweep_battery.py `directed`): mask outputs (8-bit stores)
     reused as staged 8-bit inputs, global gather / scatter / scatter_add with out-of-range indices masked off, signed
     integer operations, rounding conversions, literal operands in every position, min / max / product / count
     reductions, the guarded multiply-adds of the tape."""

@@ -3,8 +3,8 @@ of it has run on hardware yet; the file name sorts last so that `pytest -x` reac
 in round 1.
 
 GPU tests of the user-visible runtime calls of the boundary (SURVEY 8b): cuda_whos, cuda_make_managed,
-cuda_fetch_element on unevaluated variables, pre-eval callbacks, cuda_malloc_trim / cuda_mem_get_info, the kernel
-qualification verdict, and the cuda_partition device composition (opt-in path).
+cuda_fetch_element on unevaluated variables, pre-eval callbacks, cuda_malloc_trim / cuda_mem_get_info, and the
+cuda_partition device composition (opt-in path).
 Reference behaviour: src/cuda/jit.cu:455-485 (managed), :1520-1538 (fetch_element), :1421-1422 (callbacks),
 :1564-1634 (whos), :1715-1723 (trim + retry)."""
 import ctypes
@@ -78,27 +78,6 @@ def test_pre_eval_callbacks(gpu):
     b = a * 2.0
     ek.cuda_eval()
     assert len(hits) == n and b.coeff(3) == np.float32(4.0)
-
-
-def test_kernel_qualification_verdict(gpu):
-    """ek_init() decided between the fast and the general sweep kernel (csrc/ek_runtime.cpp "kernel qualification").
-    Whatever the verdict, wide 32-bit sweeps must run, be bit-exact, and use the kernel the verdict names.  When the verdict
-    is negative the helper is run once more in the foreground so that the test log shows which comparison disagreed."""
-    ek = gpu
-    L = ek.lib()
-    mode = L.ek_fast_mode()
-    x = np.random.default_rng(5).uniform(-3, 3, 300_001).astype(np.float32)
-    L.ek_stats_reset()
-    y = (ek.Float32.copy(x) * 1.25 + 0.5).numpy()
-    assert (y == x * np.float32(1.25) + np.float32(0.5)).all()
-    st = ek.stats()
-    assert int(st.sweep_launches) >= 1
-    assert (int(st.fast_launches) > 0) == bool(mode)
-    if not mode and os.environ.get("EK_FAST") is None:
-        helper = os.path.join(ROOT, "enoki_b200", "ek_qualify")
-        r = subprocess.run([helper], capture_output=True, text=True, timeout=600, env=dict(os.environ, EK_FAST="0"))
-        sys.stderr.write(r.stderr[-3000:])
-        pytest.skip("the fast sweep kernel did NOT qualify on this GPU (general kernels are in use); ek_qualify says: " + r.stderr[-1500:])
 
 
 @pytest.mark.parametrize("n,k", [(1, 1), (31, 3), (100_003, 7), (1 << 22, 40), (50_000, 1500)])
