@@ -65,8 +65,8 @@ struct Assembled {
     uint32_t n_arith = 0;
     bool has64 = false;                         /* any 64-bit value: needs the general (high-plane) kernel */
     bool noncore = false;                       /* uses an op that is compiled out of the V=16 fast kernel */
-    uint32_t release_mask = 0;                  /* staged inputs released by the EKF_REL instruction (single-stage configs) */
-    int release_at = -1;                        /* body index of that instruction */
+    uint32_t release_mask = 0;                  /* staged inputs (bit k: staged[k]) dead after body[release_at] ... */
+    int release_at = -1;                        /* ... where the fast kernel's lowering inserts its FF_REL instruction (early release) */
     uint64_t bytes_in = 0, bytes_out = 0;
     struct DescFix { uint32_t argw; uint32_t count_limit; };
     /* shared-memory 'extra' region: staged gather tables and privatised scatter_add bins; the offsets / copy counts
@@ -971,6 +971,9 @@ struct Assembler {
     void plan_release() {
         size_t ns = out.staged.size(), nb = out.body.size();
         if (ns == 0 || ns > 16 || nb < 3) return;
+        /* programs with gathers / scatters are bound by those, not by streaming their inputs: there the release's
+           barrier and extra dispatch cost more than the overlap gains (C3 measured 3-7 % slower with it on an H100) */
+        for (const EkInstr &in : out.body) if (in.op >= DOP_GATHER_32 && in.op <= DOP_SCATTER_ADD_I32_SMEM) return;
         std::vector<int> last(ns, -1);
         auto unit_of = [&](uint16_t code) -> int { return (code != EK_OPND_NONE && !(code & 0x8000u) && (code & EK_OPND_STAGED)) ? (int) (code & 0x3fffu) : -1; };
         for (size_t i = 0; i < nb; ++i) {
@@ -1234,8 +1237,9 @@ bool fop_has_u_twin(int fop) {
 }
 
 /* `in` = assembled instructions whose operand codes are still symbolic (uniform index | 0x8000, staged unit | 0x4000,
-   temporary slot); cfg == nullptr: count / check only.  Appends to `out`; false = not expressible. */
-bool lower_fast(const std::vector<EkInstr> &in, const Assembled &a, const Config *cfg, std::vector<EkInstr> &out) {
+   temporary slot); cfg == nullptr: count / check only.  Appends to `out`; false = not expressible.  release_at >= 0
+   (the body, with a.release_at): a NOP carrying FF_REL and the release mask (imm) follows what in[release_at] lowers to. */
+bool lower_fast(const std::vector<EkInstr> &in, const Assembled &a, const Config *cfg, std::vector<EkInstr> &out, int release_at = -1) {
     const uint32_t slot_bytes = cfg ? cfg->T * 16u * 4u : 0u;
     auto is_uni = [](uint16_t c) { return c != EK_OPND_NONE && (c & EK_OPND_UNI) != 0; };
     /* per-thread operand -> absolute byte offset >> 4; uniform operand -> pool word index */
@@ -1254,8 +1258,13 @@ bool lower_fast(const std::vector<EkInstr> &in, const Assembled &a, const Config
            format reads y = b | c << 16, z = dst | aux << 16 -- hence the shuffled assignment above) */
         out.push_back(o);
     };
-    for (const EkInstr &i : in) {
-        if (i.flags & (EKF_R64 | EKF_B64 | EKF_C64 | EKF_A64 | EKF_REL)) return false;
+    const size_t first = out.size();
+    /* (emitted once every instruction lowered from in[release_at] is out: at the top of the next iteration) */
+    auto mark_release = [&](size_t j) { if (release_at >= 0 && j == (size_t) release_at + 1) emit(FOP_NOP, FF_REL, 0, 0, 0, 0, a.release_mask); };
+    for (size_t j = 0; j < in.size(); ++j) {
+        mark_release(j);
+        const EkInstr &i = in[j];
+        if (i.flags & (EKF_R64 | EKF_B64 | EKF_C64 | EKF_A64)) return false;
         /* 1. accumulator load and input modifiers become instructions of their own */
         if (i.flags & EKF_HAS_A) {
             if (is_uni(i.a)) emit(FOP_LOADU, 0, enc(i.a), 0, 0, 0, 0);
@@ -1329,6 +1338,7 @@ bool lower_fast(const std::vector<EkInstr> &in, const Assembled &a, const Config
         if (i.op == DOP_NOP && !fl) continue;                    /* (a bare carrier of a load / modifier) */
         emit((uint32_t) fop, fl, b, c, dst, aux, i.imm);
     }
+    mark_release(in.size());
     return true;
 }
 
@@ -1479,7 +1489,6 @@ void dump_program(std::ostream &os, const Assembled &a, const Group &g) {
             os << " b=" << opnd_str(in.b) << " c=" << opnd_str(in.c);
             if (in.flags & EKF_STG) os << " stg";
             if (in.flags & EKF_RACC) os << " racc->s" << in.dst;
-            if (in.flags & EKF_REL) os << " rel";
             if (in.flags & EKF_ST) os << " -> s" << in.dst;
             os << " imm=0x" << std::hex << in.imm << std::dec << "\n";
         }
@@ -1533,7 +1542,7 @@ static int eval_impl(bool dry, std::string *dump, bool json = false) {
         bool ok = as.run();
         if (ok && !as.out.has64 && !as.out.noncore) {
             std::vector<EkInstr> lowered;
-            as.out.fast_ok = lower_fast(as.out.init, as.out, nullptr, lowered) && lower_fast(as.out.body, as.out, nullptr, lowered) &&
+            as.out.fast_ok = lower_fast(as.out.init, as.out, nullptr, lowered) && lower_fast(as.out.body, as.out, nullptr, lowered, as.out.release_at) &&
                              lower_fast(as.out.fini, as.out, nullptr, lowered);
             as.out.fast_len = (uint32_t) lowered.size();
         }
@@ -1598,7 +1607,7 @@ static int eval_impl(bool dry, std::string *dump, bool json = false) {
                 /* (judged as a wide sweep whatever its size, so that small CPU test cases exercise the lowering too) */
                 if (choose_config(ctx, a, std::max<size_t>(l.first->size, 4097), fcfg, ferr) && fcfg.fast) {
                     std::vector<EkInstr> fi, fb, ff;
-                    if (lower_fast(a.init, a, &fcfg, fi) && lower_fast(a.body, a, &fcfg, fb) && lower_fast(a.fini, a, &fcfg, ff)) {
+                    if (lower_fast(a.init, a, &fcfg, fi) && lower_fast(a.body, a, &fcfg, fb, a.release_at) && lower_fast(a.fini, a, &fcfg, ff)) {
                         oss << ",\"fast\":{\"T\":" << fcfg.T << ",\"off_slots\":" << fcfg.off_slots << ",\"n_tmp\":" << a.n_tmp
                             << ",\"off_bar\":" << fcfg.off_bar << ",\"off_extra\":" << fcfg.off_extra << ",\"smem\":" << fcfg.smem
                             << ",\"n_in_units\":" << a.n_in_units << ",\"n_red\":" << a.n_red << ",\"argw\":[";
@@ -1616,7 +1625,7 @@ static int eval_impl(bool dry, std::string *dump, bool json = false) {
                             oss << "]";
                         };
                         fsec("init", fi); fsec("body", fb); fsec("fini", ff);
-                        oss << "}";
+                        oss << ",\"release_mask\":" << (a.release_at >= 0 ? a.release_mask : 0u) << "}";
                     }
                 }
                 oss << "}";
@@ -1683,7 +1692,7 @@ static int eval_impl(bool dry, std::string *dump, bool json = false) {
         memset(&args, 0, sizeof(args));
         std::vector<EkInstr> lowered_init, lowered_body, lowered_fini;
         if (fast) {
-            if (!lower_fast(a.init, a, &cfg, lowered_init) || !lower_fast(a.body, a, &cfg, lowered_body) || !lower_fast(a.fini, a, &cfg, lowered_fini) ||
+            if (!lower_fast(a.init, a, &cfg, lowered_init) || !lower_fast(a.body, a, &cfg, lowered_body, a.release_at) || !lower_fast(a.fini, a, &cfg, lowered_fini) ||
                 lowered_init.size() + lowered_body.size() + lowered_fini.size() > EK_INLINE_PROG) {
                 ek_set_error("ek_eval(): internal error: fast-kernel lowering failed after it had been checked"); return -1;
             }

@@ -42,8 +42,6 @@ struct EkInstr {
 #define EKF_HAS_A 0x0080u   /* load the accumulator from operand `a` before executing        */
 #define EKF_NEG_A 0x0100u   /* f32 input modifier: accumulator = -accumulator                 */
 #define EKF_ABS_A 0x0200u   /* f32 input modifier: accumulator = |accumulator|                */
-#define EKF_REL   0x0800u   /* after executing: the staged inputs in args.release_mask are dead for this tile --
-                               start streaming them for the CTA's next tile (single-buffered pipelines)   */
 #define EKF_RACC  0x4000u   /* after executing: fold the accumulator into the reduction partials in slot dst
                                (kind | class << 8 in field `a`; only when EKF_ST and EKF_HAS_A are clear)   */
 #define EKF_STG   0x0400u   /* after executing, store the 32-bit accumulator to the global array
@@ -156,7 +154,9 @@ enum EkDop : uint16_t {
 #define FF_RACC 0x0040u   /* fold the accumulator into the reduction partials in slot dst       */
 #define FF_VU   0x0080u   /* scatters: the value operand is the uniform-pool word b             */
 #define FF_MU   0x0100u   /* gathers / scatters: the mask operand is the uniform-pool word (b for gathers, c for scatters) */
-#define FF_POST (FF_ST | FF_STG | FF_RACC)
+#define FF_REL  0x0200u   /* (on a NOP) the staged inputs in imm (bit k: staged input k) are dead for this tile -- refill
+                             their buffers with the CTA's next tile while the rest of the tile computes (early release) */
+#define FF_POST (FF_ST | FF_STG | FF_RACC | FF_REL)   /* (one test per dispatch for everything after the operation) */
 
 /* binary operations: every entry X has a twin X_U = X + 1 whose second operand is uniform-pool word b */
 #define EK_FOPS2(X) \
@@ -219,7 +219,6 @@ struct EkSweepArgs {
     uint32_t smem_prog_off;        /*   mbarriers+reduction scratch, program copy,            */
     uint32_t smem_extra_off;       /*   privatised bins / staged tables,                      */
     uint32_t smem_slots_off;       /*   slot file (1024-byte aligned)                         */
-    uint32_t release_mask;         /* staged inputs (bit k) released early by the EKF_REL instruction */
     uint32_t prog_in_smem;         /* (global-memory programs) copy the program to shared memory */
     uint32_t n_red;                /* number of reductions                                    */
     uint64_t *red_partials;        /* [n_red][grid] 8-byte partials                           */

@@ -14,13 +14,28 @@
 namespace {
 
 #ifdef EK_HOST_EMU
-/* host emulation (tests/cpu_kernel): shared-space addresses are offsets into the CTA's buffer, an mbarrier is a word
-   {bit 0: parity of the current phase, bits 32..: pending transaction bytes}, a TMA bulk copy is a memcpy */
+/* host emulation (tests/cpu_kernel): shared-space addresses are offsets into the CTA's buffer, an mbarrier (expected
+   arrival count 1) is a word {bit 0: parity of the current phase, bit 1: the phase's arrival has been made, bits 32..:
+   pending transaction bytes}, a TMA bulk copy is a memcpy.  A phase completes when it has its arrival AND no pending
+   bytes: bytes may be expected before the arrival (an early release), and then the barrier must not flip early. */
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t) __cvta_generic_to_shared(p); }
 inline uint8_t *emu_smem_ptr(uint32_t addr) { return emu::smem_ + (addr - emu::SMEM_WINDOW); }
+/* atomically apply (arrive?, +add bytes, -sub bytes) and complete the phase when it is due */
+inline void emu_mbar_update(uint64_t *bar, bool arrive, uint32_t add, uint32_t sub) {
+    uint64_t w = __atomic_load_n(bar, __ATOMIC_SEQ_CST), nw;
+    do {
+        const uint64_t tx = (w >> 32) + add;
+        if (tx < sub) emu::trap("mbarrier transaction count underflow");
+        const uint64_t left = tx - sub;
+        const bool arrived = ((w >> 1) & 1u) || arrive;
+        if (arrive && ((w >> 1) & 1u)) emu::trap("second arrival on a count-1 mbarrier phase");
+        nw = (left << 32) | (w & 1u) | (arrived ? 2u : 0u);
+        if (arrived && left == 0) nw = (w & 1u) ^ 1u;                 /* phase complete: next parity, no arrival yet */
+    } while (!__atomic_compare_exchange_n(bar, &w, nw, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST));
+}
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t) { __atomic_store_n(bar, 0ull, __ATOMIC_SEQ_CST); }
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) { __atomic_fetch_add(bar, (uint64_t) bytes << 32, __ATOMIC_SEQ_CST); }
-__device__ __forceinline__ void mbar_expect_tx_only(uint64_t *bar, uint32_t bytes) { __atomic_fetch_add(bar, (uint64_t) bytes << 32, __ATOMIC_SEQ_CST); }
+__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) { emu_mbar_update(bar, true, bytes, 0); }
+__device__ __forceinline__ void mbar_expect_tx_only(uint64_t *bar, uint32_t bytes) { emu_mbar_update(bar, false, bytes, 0); }
 __device__ __forceinline__ uint32_t mbar_try_wait(uint32_t bar_addr, uint32_t parity) {
     const uint64_t w = __atomic_load_n(reinterpret_cast<uint64_t *>(emu_smem_ptr(bar_addr)), __ATOMIC_SEQ_CST);
     return ((uint32_t) w & 1u) != parity;
@@ -33,8 +48,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) { mbar
 __device__ __forceinline__ void tma_load_1d(void *dst_smem, const void *src, uint32_t bytes, uint64_t *bar) {
     if (((uintptr_t) src & 15u) || (bytes & 15u) || (smem_u32(dst_smem) & 15u)) emu::trap("misaligned bulk copy");
     memcpy(dst_smem, src, bytes);
-    const uint64_t left = __atomic_sub_fetch(bar, (uint64_t) bytes << 32, __ATOMIC_SEQ_CST);
-    if ((left >> 32) == 0) __atomic_fetch_xor(bar, 1ull, __ATOMIC_SEQ_CST);       /* phase complete */
+    emu_mbar_update(bar, false, 0, bytes);
 }
 __device__ __forceinline__ void tma_prefetch_l2(const void *, uint32_t) {}
 __device__ __forceinline__ void fence_barrier_init() {}
