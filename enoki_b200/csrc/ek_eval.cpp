@@ -615,7 +615,18 @@ struct Assembler {
             ini.flags |= EKF_ST | (w64 ? EKF_R64 : 0); ini.dst = (uint16_t) acc;
             out.init.push_back(ini);
             EkInstr *last = out.body.empty() ? nullptr : &out.body.back();
-            if (acc_var == d0 && !pending_a && !pending_mod && last && last_emitted_for == d0 &&
+            const bool mask_red = op == EK_OP_ALL || op == EK_OP_ANY || op == EK_OP_COUNT;
+            if (mask_red) {
+                /* a borrowed mask may hold any non-zero byte for `true` (2, 0xff): fold (x != 0), so that COUNT adds 1
+                   per true element and ALL / ANY produce a canonical 0 / 1 */
+                ensure_acc(d0);
+                push_body(mk(DOP_NEZ_32));
+                acc_var = 0;
+                EkInstr in = mk(DOP_RACC, (uint32_t) kind | ((uint32_t) cls << 8));
+                in.dst = (uint16_t) acc;
+                push_body(in);
+                last_emitted_for = 0;
+            } else if (acc_var == d0 && !pending_a && !pending_mod && last && last_emitted_for == d0 &&
                 !(last->flags & (EKF_ST | EKF_HAS_A | EKF_RACC))) {
                 /* fused into the instruction that produces the value */
                 last->flags |= EKF_RACC;

@@ -258,6 +258,8 @@ class Emulator:
                 staged[unit] = np.ascontiguousarray(a).view(np.uint64)        # unpacked by LD_64
             elif es == 1:
                 staged[unit] = np.ascontiguousarray(a).view(np.uint8)         # unpacked by LD_U8 / LD_S8
+            elif es == 2:
+                staged[unit] = np.ascontiguousarray(a).view(np.uint16)        # unpacked by LD_U16 / LD_S16
             else:
                 raise Unsupported("staged input of element size %d" % es)
         out_type = {var: typ for var, _aw, _bytes, typ in sw["outputs"]}
@@ -340,14 +342,38 @@ class Emulator:
                 elif cls in (1, 2):
                     a = acc.view(np.int32 if cls == 1 else np.uint32); r = R.view(a.dtype)
                     res = {0: a + r, 1: a * r, 2: np.minimum(a, r), 3: np.maximum(a, r)}[kind]
-                else:
-                    raise Unsupported("64-bit reduction")
+                else:                                   # F64 / I64 / U64: (lo, hi) planes in slots dst, dst + 1
+                    a, r = self._j(acc, slots[slot + 1]), self._j(R, state["Rh"])
+                    if cls == 3 and kind >= 2:          # red_combine: min_x86(y, x)
+                        x, y = np.ascontiguousarray(r.view(np.float64)), np.ascontiguousarray(a.view(np.float64))
+                        res = np.zeros_like(x)
+                        self.oracle.or_minmax_f64(int(kind == 3), _P(x), _P(y), _P(res), SZ(len(x)))
+                    elif cls == 3:
+                        a, r = a.view(np.float64), r.view(np.float64)
+                        res = a + r if kind == 0 else a * r
+                    elif kind <= 1:
+                        res = a + r if kind == 0 else a * r
+                    else:
+                        dt = np.int64 if cls == 4 else np.uint64
+                        res = (np.minimum if kind == 2 else np.maximum)(a.view(dt), r.view(dt))
+                    slots[slot], slots[slot + 1] = self._s(res)
+                    return
             slots[slot] = self._u(np.ascontiguousarray(res))
 
-        def rfin(B, imm, dst):
+        def rfin(B, Bh, imm, dst):
             kind, cls = imm & 0xff, (imm >> 8) & 0xff
             if cls > 2:
-                raise Unsupported("64-bit reduction")
+                x = self._j(B, Bh)
+                if cls == 3:
+                    x = x.view(np.float64)
+                    val = np.array([{0: x.sum(), 1: np.prod(x), 2: x.min(), 3: x.max()}[kind]], np.float64)
+                else:
+                    dt = np.int64 if cls == 4 else np.uint64
+                    r = {0: lambda: np.sum(x, dtype=np.uint64), 1: lambda: np.multiply.reduce(x),
+                         2: lambda: x.view(dt).min(), 3: lambda: x.view(dt).max()}[kind]()
+                    val = np.array([r]).astype(dt)
+                self.vars[var_of_uniform(dst)] = val
+                return
             if cls == 0:
                 x = self._f(B).astype(np.float64)
                 r = {0: x.sum(), 1: np.prod(x), 2: x.min(), 3: x.max()}[kind]
@@ -468,6 +494,9 @@ class Emulator:
                 elif name in ("LD_U8", "LD_S8"):
                     v = staged[cb & 0x3fff]
                     R = v.astype(np.uint32) if name == "LD_U8" else v.view(np.int8).astype(np.int32).view(np.uint32)
+                elif name in ("LD_U16", "LD_S16"):
+                    v = staged[cb & 0x3fff]
+                    R = v.astype(np.uint32) if name == "LD_U16" else v.view(np.int16).astype(np.int32).view(np.uint32)
                 elif name == "ST_8":
                     var = var_of_uniform(imm)
                     self.vars[var] = (R & 0xff).astype(np.uint8).view(np.bool_) if out_type.get(var) == T_BOOL else (R & 0xff).astype(np.uint8)
@@ -545,7 +574,7 @@ class Emulator:
                         self.vars[var] = tgt.view(self.vars[var].dtype)
                     return
                 elif name == "RACC": state["R"] = R; racc(dst, imm); return
-                elif name == "RFIN": rfin(B, imm, dst); return
+                elif name == "RFIN": rfin(B, Bh, imm, dst); return
                 else:
                     raise Unsupported(name)
             state["R"] = np.ascontiguousarray(R).astype(np.uint32, copy=False)
