@@ -767,7 +767,11 @@ struct Assembler {
                     out.argw.push_back(out.extra_bytes); out.argw.push_back(count); out.argw.push_back(copies); out.argw.push_back(pa);
                     out.extra_bytes += (count * copies * 4 + 15) & ~15u;
                     out.extra_items.push_back({ di, count, (uint8_t) (dop == DOP_SCATTER_ADD_F32 ? 1 : 2) });
-                    EkInstr zi = mk(DOP_SMEM_ZERO, di); set_mark(zi, 1); out.init.push_back(zi);
+                    /* float bins start at -0.0, not +0.0: x + -0.0 == x for every x, so a bin that receives nothing (or
+                       only -0.0) leaves a -0.0 target element as it is, and the flush skips exactly those bins */
+                    EkInstr zi = mk(DOP_SMEM_ZERO, di); set_mark(zi, 1);
+                    zi.dst = dop == DOP_SCATTER_ADD_F32 ? 1 : 0;
+                    out.init.push_back(zi);
                     EkInstr fl = mk(dop == DOP_SCATTER_ADD_F32 ? DOP_SMEM_FLUSH_ADD_F32 : DOP_SMEM_FLUSH_ADD_I32, di); set_mark(fl, 1);
                     out.fini.push_back(fl);
                     in = mk(dop == DOP_SCATTER_ADD_F32 ? DOP_SCATTER_ADD_F32_SMEM : DOP_SCATTER_ADD_I32_SMEM, di); set_mark(in, 1);
@@ -1327,6 +1331,9 @@ bool lower_fast(const std::vector<EkInstr> &in, const Assembled &a, const Config
                 break;
             case DOP_RFIN:                                        /* b = slot of the partials, dst = pool index of the pointer */
                 if (!hb || ub) return false;
+                dst = i.dst;
+                break;
+            case DOP_SMEM_ZERO:                                   /* dst = 1: float bins (filled with -0.0) */
                 dst = i.dst;
                 break;
             default:

@@ -47,6 +47,10 @@ struct EkInstr {
 #define EKF_STG   0x0400u   /* after executing, store the 32-bit accumulator to the global array
                                whose pointer is the uniform pair at index imm                 */
 
+/* largest gather / scatter stride in bytes: it travels in the 15-bit field of imm (stride << 16); ek_trace_append
+   refuses larger ones */
+#define EK_MAX_GS_STRIDE 0x7fffu
+
 /* rounding modes for DOP_CVT_* (imm) */
 #define EK_RZ 0
 #define EK_RM 1
@@ -126,7 +130,7 @@ struct EkInstr {
        RFIN: b = accumulator slot, dst = uniform index of result pointer, imm = kind|class<<8|red_index<<16 */ \
     X(RACC) X(RFIN) \
     /* init/fini helpers for privatised scatter_add bins and staged gather tables \
-       (imm = descriptor index in the uniform pool) */ \
+       (imm = descriptor index in the uniform pool; SMEM_ZERO: dst = 1 for float bins, which start at -0.0) */ \
     X(SMEM_ZERO) X(SMEM_LOAD_TABLE) X(SMEM_FLUSH_ADD_F32) X(SMEM_FLUSH_ADD_I32)
 
 enum EkDop : uint16_t {

@@ -508,6 +508,15 @@ uint32_t ek_trace_append(ek_type type, ek_op op, uint32_t a, uint32_t b, uint32_
         ek_set_error("ek_trace_append(): scatter target must be a pointer registered with ek_var_register_ptr()");
         return 0;
     }
+    if (op == EK_OP_GATHER || op == EK_OP_SCATTER || op == EK_OP_SCATTER_ADD) {
+        /* the sweep program carries the stride in 15 bits: refuse what would wrap instead of addressing wrong elements */
+        const uint64_t stride = op == EK_OP_GATHER ? imm : imm >> 32;
+        if (stride > EK_MAX_GS_STRIDE) {
+            ek_set_error("ek_trace_append(): " + std::string(ek_op_name(op)) + " stride of " + std::to_string(stride) +
+                         " bytes exceeds the limit of " + std::to_string(EK_MAX_GS_STRIDE) + " bytes");
+            return 0;
+        }
+    }
     /* x / (+-2^k) == x * (+-2^-k) bit for bit (an exact scaling rounds the same real number), and the multiply is one
        instruction where div.rn is a Newton iteration with a slow-path branch: rewrite divisions by power-of-two
        literals (C3's `* 31 / 8`) */

@@ -10,6 +10,7 @@ import numpy as np
 
 F_ST, F_R64, F_HAS_B, F_HAS_C, F_B64, F_C64, F_A64, F_HAS_A, F_NEG_A, F_ABS_A, F_STG, F_RACC = 1, 2, 4, 8, 0x10, 0x20, 0x40, 0x80, 0x100, 0x200, 0x400, 0x4000
 OP_NONE = 0xFFFF
+NEG_ZERO = 0x80000000                      # bits of -0.0f, the start value of float scatter_add bins
 SZ = ctypes.c_size_t
 T_FLOAT32, T_INT32, T_UINT32, T_BOOL, T_INT64, T_UINT64, T_FLOAT64 = 10, 5, 6, 12, 7, 8, 11
 
@@ -67,6 +68,8 @@ def raise_fast(fast, fop_names, op_index):
             if fl & FF_MU: flags |= F_HAS_C; cc = uni(c)
         elif name == "RFIN":
             flags |= F_HAS_B; cb = slot(b); d = dst
+        elif name == "SMEM_ZERO":
+            d = dst
         if fl & FF_ST: flags |= F_ST; d = slot(dst)
         if fl & FF_STG: flags |= F_STG
         if fl & FF_RACC:
@@ -540,15 +543,17 @@ class Emulator:
                 elif name == "CVT_U32_F32": R = self._u(R.astype(np.float32))
                 elif name == "LDG_32": R = self._u(self.vars[var_of_uniform(imm)]).copy()
                 elif name == "ST_32": store_var(var_of_uniform(imm), R)
-                elif name == "SMEM_ZERO":
-                    cnt, _var = desc(imm); smem[imm] = np.zeros(cnt, np.uint32); return
+                elif name == "SMEM_ZERO":                    # dst = 1: float bins, which start at -0.0
+                    cnt, _var = desc(imm); smem[imm] = np.full(cnt, NEG_ZERO if dst else 0, np.uint32); return
                 elif name == "SMEM_LOAD_TABLE":
                     cnt, var = desc(imm); smem[imm] = self._u(self.vars[var])[:cnt].copy(); return
                 elif name in ("SMEM_FLUSH_ADD_F32", "SMEM_FLUSH_ADD_I32"):
                     cnt, var = desc(imm)
                     tgt = self._u(self.vars[var]).copy()
-                    if name.endswith("F32"): tgt[:cnt] = self._u(f(tgt[:cnt]) + f(smem[imm]))
-                    else: tgt[:cnt] = tgt[:cnt] + smem[imm]
+                    bins = smem[imm]
+                    if name.endswith("F32"):             # a bin still holding -0.0 adds nothing and is skipped
+                        tgt[:cnt] = np.where(bins != NEG_ZERO, self._u(f(tgt[:cnt]) + f(bins)), tgt[:cnt])
+                    else: tgt[:cnt] = tgt[:cnt] + bins
                     self.vars[var] = tgt.view(self.vars[var].dtype)
                     return
                 elif name == "GATHER_32_SMEM":
