@@ -64,7 +64,6 @@ struct Assembled {
     uint32_t extra_bytes = 0;
     uint32_t n_arith = 0;
     bool has64 = false;                         /* any 64-bit value: needs the general (high-plane) kernel */
-    bool noncore = false;                       /* uses an op that is compiled out of the V=16 fast kernel */
     uint32_t release_mask = 0;                  /* staged inputs (bit k: staged[k]) dead after body[release_at] ... */
     int release_at = -1;                        /* ... where the fast kernel's lowering inserts its FF_REL instruction (early release) */
     uint64_t bytes_in = 0, bytes_out = 0;
@@ -74,7 +73,8 @@ struct Assembled {
        region out for its block size (layout_extra) */
     struct ExtraItem { uint32_t di; uint32_t count; uint8_t kind; };   /* kind 0 table, 1 float bins, 2 integer bins */
     std::vector<ExtraItem> extra_items;
-    bool fast_ok = false;                       /* every instruction has a fast-kernel form (lower_fast) */
+    bool fast_ok = false;                       /* (programs without 64-bit values) every instruction has a fast-kernel form:
+                                                   lower_fast, which takes the fast kernel's operation set from fop_of */
     uint32_t fast_len = 0;                      /* number of lowered instructions */
     std::string error;
     bool resource_error = false;     /* a limit was hit: the caller may split the group and retry */
@@ -82,6 +82,7 @@ struct Assembled {
 
 #define EK_STAGE_UNIT_BUDGET 8u     /* slot units of TMA-staged inputs per pipeline stage */
 
+/* V = elements per thread: 16 on the fast kernel, 8 or 4 on the general kernel (ek_sweep.cu) */
 struct Config { int V; uint32_t T; uint32_t stages; uint32_t ctas_per_sm; size_t smem; uint32_t off_bar, off_prog, off_extra, off_slots; bool prog_in_smem;
                 bool fast = false;   /* the 32-bit fast kernel (ek_sweep_fast.cu) with its own program form and extra-region layout */ };
 
@@ -1058,19 +1059,6 @@ struct Assembler {
         };
         fix(out.init); fix(out.body); fix(out.fini);
         plan_release();
-        for (const EkInstr &in : out.body) {
-            switch (in.op) {
-                case DOP_DIV_I32: case DOP_DIVR_I32: case DOP_DIV_U32: case DOP_DIVR_U32: case DOP_MOD_I32: case DOP_MODR_I32:
-                case DOP_MOD_U32: case DOP_MODR_U32: case DOP_MULHI_I32: case DOP_MULHI_U32: case DOP_POPC_32: case DOP_CLZ_32:
-                case DOP_CTZ_32: case DOP_SEXT8: case DOP_SEXT16: case DOP_ZEXT8: case DOP_ZEXT16: case DOP_SHLR_32:
-                case DOP_SHRR_I32: case DOP_SHRR_U32: case DOP_MINR_F32: case DOP_MAXR_F32: case DOP_DIVR_F32:
-                case DOP_LD_U16: case DOP_LD_S16: case DOP_LDG_U8: case DOP_LDG_S8: case DOP_LDG_U16: case DOP_LDG_S16:
-                case DOP_ST_16: case DOP_GATHER_U8: case DOP_GATHER_S8: case DOP_GATHER_U16: case DOP_GATHER_S16:
-                case DOP_SCATTER_8: case DOP_SCATTER_16:
-                    out.noncore = true; break;
-                default: break;
-            }
-        }
         /* descriptors hold the uniform code of their pointer in word 3: convert to a plain index */
         for (EkInstr &in : out.init) {
             if (in.op == DOP_SMEM_ZERO || in.op == DOP_SMEM_LOAD_TABLE) {
@@ -1368,26 +1356,13 @@ bool choose_config(const EkContext &ctx, const Assembled &a, size_t n, Config &c
     /* the 32-bit fast kernel: V = 16, one TMA stage (the other CTAs of the SM hide the load) */
     static const Cand fast_cands[] = { { 16, 256, 1, 2 }, { 16, 128, 1, 4 }, { 16, 128, 1, 3 }, { 16, 128, 1, 2 }, { 16, 256, 1, 1 }, { 16, 128, 1, 1 } };
     static const Cand cands[] = {
-        /* single-buffered staging with more resident CTAs first, double buffering after: the other CTAs of the
-           SM hide the TMA latency and 16 warps hide the interpreter's dependent-issue latency
-           (tools/cfgsweep.sh times the alternatives on the GPU at hand) */
-        { 16, 256, 1, 2 }, { 16, 128, 1, 4 }, { 16, 128, 1, 3 }, { 16, 128, 2, 2 }, { 16, 128, 1, 2 },
-        { 16, 256, 2, 1 }, { 16, 128, 1, 1 },                               /* 32-bit-only programs, general kernel */
+        /* the general kernel: single-buffered staging with more resident CTAs first, double buffering after: the
+           other CTAs of the SM hide the TMA latency and 16 warps hide the interpreter's dependent-issue latency */
         { 8, 256, 1, 4 }, { 8, 256, 1, 3 }, { 8, 256, 2, 2 }, { 8, 256, 1, 2 }, { 8, 256, 2, 1 }, { 8, 256, 1, 1 },
         { 8, 128, 1, 2 }, { 8, 128, 2, 1 }, { 8, 128, 1, 1 },
         { 4, 128, 2, 1 }, { 4, 64, 2, 1 }, { 4, 32, 2, 1 } };
-    size_t n_prog = a.init.size() + a.body.size() + a.fini.size();
-    const bool core16_ok = !a.has64 && !a.noncore && n_prog <= EK_INLINE_PROG;          /* general V = 16 kernel */
-    const bool fast_ok = ctx.fast_mode != 0 && !a.has64 && !a.noncore && a.fast_ok && a.fast_len <= EK_INLINE_PROG;
+    const bool fast_ok = ctx.fast_mode != 0 && !a.has64 && a.fast_ok && a.fast_len <= EK_INLINE_PROG;
     cfg.fast = false;
-    /* tuning aid: EK_CFG="V,T,stages,ctas_per_sm" forces a configuration for wide sweeps (general kernels) */
-    if (const char *env = getenv("EK_CFG")) {
-        int V, T, S, C;
-        if (n > 4096 && sscanf(env, "%d,%d,%d,%d", &V, &T, &S, &C) == 4 && (V != 16 || core16_ok)) {
-            cfg.V = V; cfg.T = (uint32_t) T; cfg.stages = (uint32_t) S; cfg.ctas_per_sm = (uint32_t) C;
-            if (smem_layout(a, cfg, n_uni) <= budget) return true;
-        }
-    }
     if (n <= 4096) {
         /* tiny sweeps (incl. the size-1 scalar groups): one small CTA */
         static const Cand small[] = { { 4, 32, 2, 1 }, { 4, 128, 2, 1 }, { 8, 256, 2, 1 } };
@@ -1413,7 +1388,6 @@ bool choose_config(const EkContext &ctx, const Assembled &a, size_t n, Config &c
         cfg.fast = false;
     }
     for (const Cand &c : cands) {
-        if (c.V == 16 && !core16_ok) continue;
         cfg.V = c.V; cfg.T = c.T; cfg.stages = a.n_in_units ? c.stages : 2; cfg.ctas_per_sm = c.want_ctas;
         size_t need = smem_layout(a, cfg, n_uni);
         if (need > budget) continue;
@@ -1558,7 +1532,7 @@ static int eval_impl(bool dry, std::string *dump, bool json = false) {
         if (g.size > 0xffffffffull) { asm_error = "arrays with more than 2^32-1 entries are not supported (jit.cu:1066,1090)"; return false; }
         Assembler as(ctx, g, plan.forced, dry);
         bool ok = as.run();
-        if (ok && !as.out.has64 && !as.out.noncore) {
+        if (ok && !as.out.has64) {
             std::vector<EkInstr> lowered;
             as.out.fast_ok = lower_fast(as.out.init, as.out, nullptr, lowered) && lower_fast(as.out.body, as.out, nullptr, lowered, as.out.release_at) &&
                              lower_fast(as.out.fini, as.out, nullptr, lowered);
@@ -1780,8 +1754,7 @@ static int eval_impl(bool dry, std::string *dump, bool json = false) {
         if (fast) {
             ek_cuda_check(ek_launch_sweep_fast(args, grid, cfg.T, cfg.smem, ctx.stream));
         } else {
-            const bool core32 = !a.has64 && !a.noncore && inline_prog;     /* 32-bit-only program: kernels without high planes */
-            ek_cuda_check(ek_launch_sweep(cfg.V, inline_prog, core32, args, grid, cfg.T, cfg.smem, ctx.stream));
+            ek_cuda_check(ek_launch_sweep(cfg.V, inline_prog, args, grid, cfg.T, cfg.smem, ctx.stream));
         }
         if (ctx.timing) {
             ek_cuda_check(cudaEventRecord(ctx.ev_stop, ctx.stream));

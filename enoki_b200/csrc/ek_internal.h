@@ -101,7 +101,7 @@ void ek_cuda_check_impl(cudaError_t err, const char *file, int line);
 #define ek_cuda_check(x) ek_cuda_check_impl((x), __FILE__, __LINE__)
 
 /* kernels (defined in .cu files) */
-cudaError_t ek_launch_sweep(int V, bool inline_prog, bool core32, const EkSweepArgs &args, unsigned grid, unsigned block,
+cudaError_t ek_launch_sweep(int V, bool inline_prog, const EkSweepArgs &args, unsigned grid, unsigned block,
                             size_t smem_bytes, cudaStream_t stream);
 /* 32-bit fast kernel (ek_sweep_fast.cu): args.prog_inline holds the lowered program; block = 128 or 256 */
 cudaError_t ek_launch_sweep_fast(const EkSweepArgs &args, unsigned grid, unsigned block, size_t smem_bytes, cudaStream_t stream);

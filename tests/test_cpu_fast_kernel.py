@@ -202,6 +202,77 @@ def test_remaining_operations_numpy_vs_host_compiled_kernel(ek, oracle, P, n):
     gc.collect()
 
 
+# device operation -> a wide 32-bit program that needs it; none of these has a fast-kernel form
+_GENERAL_ONLY = {
+    "DIV_I32": lambda E, a: a(E.Int32) // a(E.Int32),
+    "DIV_U32": lambda E, a: a(E.UInt32) // a(E.UInt32),
+    "MOD_I32": lambda E, a: a(E.Int32) % a(E.Int32),
+    "MOD_U32": lambda E, a: a(E.UInt32) % a(E.UInt32),
+    "MULHI_I32": lambda E, a: E.mulhi(a(E.Int32), a(E.Int32)),
+    "MULHI_U32": lambda E, a: E.mulhi(a(E.UInt32), a(E.UInt32)),
+    "POPC_32": lambda E, a: E.popcnt(a(E.UInt32)),
+    "CLZ_32": lambda E, a: E.lzcnt(a(E.UInt32)),
+    "CTZ_32": lambda E, a: E.tzcnt(a(E.UInt32)),
+    "SEXT8": lambda E, a: a(E.Int8) + a(E.Int8),                   # (8-bit staged loads and stores do have a form)
+    "ZEXT8": lambda E, a: a(E.UInt8) + a(E.UInt8),
+    "LD_U16": lambda E, a: E.UInt32(a(E.UInt16)) + 1,
+    "ST_16": lambda E, a: E.UInt16(a(E.UInt8)),
+    "GATHER_U8": lambda E, a: E.gather(E.UInt8, a(E.UInt8), a(E.UInt32)),
+    "SCATTER_8": lambda E, a: E.scatter(a(E.UInt8), E.UInt8(3), a(E.UInt32)),
+    "SCATTER_16": lambda E, a: E.scatter(a(E.UInt16), E.UInt16(3), a(E.UInt32)),
+}
+
+
+def _c2(E, a):
+    x0, x1, x2, x3 = (a(E.Float32) for _ in range(4))
+    t = E.fmadd(x0, x1, x2)
+    return E.fmadd(E.sin(E.fmadd(x3, E.exp(-(t * t)), x0)), x1, E.sqrt(abs(t)))
+
+
+def _c3(E, a):
+    tab, bins, hist = a(E.Float32, 31), a(E.UInt32, 31), a(E.Float32, 31)
+    idx = E.UInt32((a(E.Float32) + 4.0) * 31.0 / 8.0)
+    mask = idx < E.UInt32(31)
+    w = E.gather(E.Float32, tab, idx, mask)
+    E.scatter_add(bins, E.UInt32(1), idx, mask)
+    E.scatter_add(hist, w, idx, mask)
+
+
+@pytest.mark.parametrize("case", [*_GENERAL_ONLY, "C2", "C3", "C2_fast_mode_off"])
+def test_which_programs_the_fast_kernel_runs(ek, case):
+    """The fast kernel's operation set is what lower_fast can lower (fop_of in ek_eval.cpp): a wide 32-bit program that
+    uses one operation outside it runs on the general kernel as a whole, so its sweep in ek_debug_program() has no "fast"
+    section.  C2 and C3 lower, unless ek_set_fast_mode(0) has switched the fast kernel off."""
+    import gc
+    gc.collect(); ek.lib().ek_debug_discard_side_effects(); gc.collect()
+    n = 5000                                        # wide: n > 4096
+    mapped = []
+
+    def a(cls, size=n):                             # a mapped array (the program is planned, never run)
+        mapped.append(cls.map(0x770000000000 +0x1000000 * len(mapped), size))
+        return mapped[-1]
+    build = _GENERAL_ONLY.get(case) or (_c3 if case == "C3" else _c2)
+    L = ek.lib()
+    old = L.ek_fast_mode()
+    try:
+        L.ek_set_fast_mode(0 if case == "C2_fast_mode_off" else 1)
+        out = build(ek, a)
+        prog = ek.debug_program()
+    finally:
+        L.ek_set_fast_mode(old)
+    sweeps = [sw for sw in prog["sweeps"] if sw["n"] == n]
+    assert len(sweeps) == 1
+    sw = sweeps[0]
+    if case in _GENERAL_ONLY:
+        ops = {prog["ops"][t[0]] for sec in ("init", "body", "fini") for t in sw[sec]}
+        assert case in ops, ops
+        assert "fast" not in sw
+    else:
+        assert ("fast" in sw) == (case != "C2_fast_mode_off")
+    del out, mapped
+    L.ek_debug_discard_side_effects()
+
+
 def test_block_size_128_instantiation():
     """The same cases once more with the fast kernel restricted to its 128-thread instantiation (EK_FAST_T=128 is read once
     per process, hence the child process): operand offsets, group strides and the reduction epilogue for T = 128."""
