@@ -342,6 +342,38 @@ def scatter_add(target, value, index, mask=True):
     _scatter("SCATTER_ADD", target, value, index, mask)
 
 
+def partition(ptrs):
+    """Virtual-call dispatch grouping of a UInt64 pointer array (CUDAArray<T *>::partition_(), cuda.h:814-843):
+    [(pointer, UInt32 indices holding it)], pointers ascending, indices ascending inside a group."""
+    if ptrs.Type != EK_UINT64:
+        raise TypeError("partition(): expects a UInt64 array")
+    ptrs.eval()
+    L = lib()
+    uniq, counts, lists = ctypes.c_void_p(), ctypes.c_void_p(), ctypes.c_void_p()
+    _check(0, L.ek_partition(ptrs.size(), ptrs.data(), ctypes.byref(uniq), ctypes.byref(counts),
+                             ctypes.byref(lists)) == 0)
+    try:
+        k = ctypes.cast(counts, ctypes.POINTER(ctypes.c_uint32))[0]
+        sizes = np.ctypeslib.as_array(ctypes.cast(counts, ctypes.POINTER(ctypes.c_uint32)), shape=(k + 1,))[1:].copy()
+        keys = np.ctypeslib.as_array(ctypes.cast(uniq, ctypes.POINTER(ctypes.c_uint64)), shape=(k,)).copy()
+        ptrs_d = np.ctypeslib.as_array(ctypes.cast(lists, ctypes.POINTER(ctypes.c_uint64)), shape=(k,)).copy()
+    finally:
+        L.ek_host_free(uniq)
+        L.ek_host_free(counts)
+    try:
+        groups = []
+        for g in range(k):                 # each list is owned by its UInt32 from here on (dealloc = true)
+            groups.append((int(keys[g]), UInt32.map(int(ptrs_d[g]), int(sizes[g]), True)))
+            ptrs_d[g] = 0
+    finally:
+        for p in ptrs_d[ptrs_d != 0]:
+            L.ek_free(ctypes.c_void_p(int(p)))
+        libc = ctypes.CDLL(None)
+        libc.free.argtypes = [ctypes.c_void_p]
+        libc.free(lists)
+    return groups
+
+
 def cuda_eval():
     _check(0, lib().ek_eval() == 0)
 

@@ -18,7 +18,7 @@ class ek_stats(ctypes.Structure):
     _fields_ = [("launches", c_u64), ("sweep_launches", c_u64), ("adjoint_launches", c_u64),
                 ("ops_evaluated", c_u64), ("edge_adjoints", c_u64), ("bytes_in", c_u64),
                 ("bytes_out", c_u64), ("last_kernel_ms", ctypes.c_float),
-                ("total_kernel_ms", ctypes.c_float), ("fast_launches", c_u64)]
+                ("total_kernel_ms", ctypes.c_float), ("fast_launches", c_u64), ("partition_device", c_u64)]
 
 
 # name -> (restype, argtypes); every symbol include/enoki_b200.h declares

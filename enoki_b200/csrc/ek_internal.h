@@ -108,6 +108,8 @@ cudaError_t ek_launch_sweep_fast(const EkSweepArgs &args, unsigned grid, unsigne
 void ek_launch_fill(void *ptr, size_t elem_size, uint64_t value, size_t n, cudaStream_t stream);
 void ek_launch_reverse(void *out, const void *in, size_t elem_size, size_t n, cudaStream_t stream);
 void ek_launch_flush(void *buf, size_t bytes, cudaStream_t stream);
+/* inclusive prefix sum of n uint32 values on the runtime's stream (ek_scan.cu: the three-phase scan of ek_psum) */
+void ek_scan_incl_u32(const uint32_t *in, uint32_t *out, size_t n);
 
 /* type helpers */
 static inline size_t ek_type_size(ek_type t) {

@@ -108,17 +108,21 @@ tile_compact(const T *in, const uint8_t *mask, T *out, const uint32_t *tile_off,
 struct ConvId { template <typename T> __device__ T operator()(T v) const { return v; } };
 struct ConvFlag { __device__ uint32_t operator()(uint8_t v) const { return v ? 1u : 0u; } };
 
-template <typename T> void *psum_impl(size_t n, const void *data) {
+template <typename T> void scan_incl(const T *in, T *out, size_t n) {
     EkContext &ctx = ek_ctx();
     size_t n_tiles = (n + TILE - 1) / TILE;
     T *tile = (T *) ek_malloc(n_tiles * sizeof(T));
-    T *out = (T *) ek_malloc(n * sizeof(T));
-    tile_reduce<T, T, ConvId><<<(unsigned) n_tiles, THREADS, 0, ctx.stream>>>((const T *) data, tile, n, ConvId());
+    tile_reduce<T, T, ConvId><<<(unsigned) n_tiles, THREADS, 0, ctx.stream>>>(in, tile, n, ConvId());
     scan_tile_sums<T><<<1, THREADS, 0, ctx.stream>>>(tile, n_tiles);
-    tile_scan_incl<T><<<(unsigned) n_tiles, THREADS, 0, ctx.stream>>>((const T *) data, out, tile, n);
+    tile_scan_incl<T><<<(unsigned) n_tiles, THREADS, 0, ctx.stream>>>(in, out, tile, n);
     ek_cuda_check(cudaGetLastError());
     ctx.stats.launches += 3;
     ek_free(tile);
+}
+
+template <typename T> void *psum_impl(size_t n, const void *data) {
+    T *out = (T *) ek_malloc(n * sizeof(T));
+    scan_incl<T>((const T *) data, out, n);
     return out;
 }
 
@@ -146,6 +150,8 @@ template <typename T> int compress_impl(size_t n, const void *data, const uint8_
 
 } // namespace
 
+void ek_scan_incl_u32(const uint32_t *in, uint32_t *out, size_t n) { scan_incl<uint32_t>(in, out, n); }
+
 extern "C" {
 
 void *ek_psum(ek_type type, size_t n, const void *data) {
@@ -170,137 +176,6 @@ int ek_compress(ek_type type, size_t n, const void *data, const uint8_t *mask, v
         case 8: return compress_impl<uint64_t>(n, data, mask, out_data, out_size);
         default: ek_set_error("ek_compress(): unsupported type"); return -1;
     }
-}
-
-/* cuda_partition (horiz.cu:35-122): groups the indices 0..n-1 by pointer value -- unique pointers ascending, indices
-   ascending inside every group (what the reference's stable radix sort + run-length encode produce).
-
-   Default path (round 2): the pointer array is downloaded and grouped by a host-side stable sort; the per-group index
-   lists are uploaded.  This is NOT a performance path (virtual-call dispatch is a "next" row of SURVEY 8f, its cost is
-   dominated by the per-instance kernels) and it is the only variant that could be reasoned correct without hardware:
-   this repository lost its GPU access before any device-side variant had been seen to pass.
-   EK_PARTITION_DEVICE=1 selects a device-side composition of primitives the parity tests already pin -- no kernel of
-   its own:
-     (1) distinct values, ascending:  v_0 = hmin(ptr);  v_{k+1} = hmin(select(ptr > v_k, ptr, ~0))   (fused sweep +
-         reduction epilogue, one 8-byte read-back per value),
-     (2) per value: mask = (ptr == v_k) recorded through the evaluator, indices = compress(arange(n), mask)
-         (ek_compress: three-phase scan, output order = input order, i.e. ascending).
-   Cost: 2 K passes over the pointer array for K distinct values; more than EK_PART_MAX_GROUPS distinct values fall back
-   to the host sort.
-
-   History: round 1 shipped a dedicated hash + multi-way scatter kernel set; every GPU box that ran its test was lost
-   after ~2 minutes.  The cause found in round 2 was the TEST, not the kernels: it built its pointer table with
-   rng.choice(np.arange(1, 1 << 40)) -- an 8 TiB host allocation that took the box down (tests/test_gpu_eval.py
-   test_partition, fixed).  The kernel set was removed before that was understood and has not been brought back. */
-namespace {
-constexpr size_t EK_PART_MAX_GROUPS = 256;
-
-struct Handle {             /* scoped external reference on a trace variable */
-    uint32_t h = 0;
-    Handle() = default;
-    explicit Handle(uint32_t v) : h(v) {}
-    Handle(const Handle &) = delete; Handle &operator=(const Handle &) = delete;
-    Handle(Handle &&o) noexcept : h(o.h) { o.h = 0; }
-    Handle &operator=(Handle &&o) noexcept { if (this != &o) { reset(); h = o.h; o.h = 0; } return *this; }
-    ~Handle() { reset(); }
-    void reset() { if (h) ek_dec_ref_ext(h); h = 0; }
-    explicit operator bool() const { return h != 0; }
-};
-
-int partition_host_sort(EkContext &ctx, size_t n, const uint64_t *keys, std::vector<uint64_t> &uniq,
-                        std::vector<uint32_t> &cnts, uint32_t **&perm_h) {
-    std::vector<uint64_t> hk(n);
-    ek_cuda_check(cudaMemcpyAsync(hk.data(), keys, n * 8, cudaMemcpyDeviceToHost, ctx.stream));
-    ek_cuda_check(cudaStreamSynchronize(ctx.stream));
-    std::vector<uint32_t> order(n);
-    for (size_t i = 0; i < n; ++i) order[i] = (uint32_t) i;
-    std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return hk[a] < hk[b]; });
-    std::vector<size_t> starts;
-    for (size_t i = 0; i < n; ++i) if (i == 0 || hk[order[i]] != hk[order[i - 1]]) { starts.push_back(i); uniq.push_back(hk[order[i]]); }
-    starts.push_back(n);
-    perm_h = (uint32_t **) malloc(sizeof(uint32_t *) * uniq.size());
-    for (size_t k = 0; k < uniq.size(); ++k) {
-        uint32_t c = (uint32_t) (starts[k + 1] - starts[k]);
-        cnts.push_back(c);
-        perm_h[k] = (uint32_t *) ek_malloc((size_t) c * 4);
-        ek_cuda_check(cudaMemcpyAsync(perm_h[k], order.data() + starts[k], (size_t) c * 4, cudaMemcpyHostToDevice, ctx.stream));
-    }
-    ek_cuda_check(cudaStreamSynchronize(ctx.stream));
-    return 0;
-}
-} // namespace
-
-int ek_partition(size_t n, const void **ptrs, void ***unique_out, uint32_t **counts_out, uint32_t ***perm_out) {
-    if (ek_init() != 0) return -1;
-    EkContext &ctx = ek_ctx();
-    if (n == 0 || n > 0xffffffffull) { ek_set_error("ek_partition(): unsupported size"); return -1; }
-    const uint64_t *keys = reinterpret_cast<const uint64_t *>(ptrs);
-    std::vector<uint64_t> uniq;
-    std::vector<uint32_t> cnts;
-    uint32_t **perm_h = nullptr;
-    bool host = getenv("EK_PARTITION_DEVICE") == nullptr;
-
-    if (!host) {
-        /* borrow the caller's array as a trace variable (jit.cu:373-395 with dealloc = false) */
-        Handle kv(ek_var_register(EK_UINT64, n, const_cast<void *>((const void *) ptrs), 0));
-        if (!kv) return -1;
-        auto lit64 = [](uint64_t v) { return Handle(ek_trace_append(EK_UINT64, EK_OP_LITERAL, 0, 0, 0, v)); };
-        /* (1) distinct values in ascending order */
-        bool have_prev = false; uint64_t prev = 0;
-        while (true) {
-            Handle m;
-            if (!have_prev) {
-                m = Handle(ek_trace_append(EK_UINT64, EK_OP_HMIN, kv.h, 0, 0, 0));
-            } else {
-                Handle lp = lit64(prev), top = lit64(~0ull);
-                Handle gt(ek_trace_append(EK_BOOL, EK_OP_GT, kv.h, lp.h, 0, 0));
-                if (!lp || !top || !gt) return -1;
-                Handle cand(ek_trace_append(EK_UINT64, EK_OP_SELECT, gt.h, kv.h, top.h, 0));
-                if (!cand) return -1;
-                m = Handle(ek_trace_append(EK_UINT64, EK_OP_HMIN, cand.h, 0, 0, 0));
-            }
-            if (!m || ek_eval_var(m.h) != 0) return -1;
-            uint64_t v = 0;
-            if (ek_fetch_element(&v, m.h, 0, 8) != 0) return -1;
-            if (have_prev && v == ~0ull) break;
-            uniq.push_back(v); prev = v; have_prev = true;
-            if (v == ~0ull) break;                         /* (not a pointer value; nothing can follow it) */
-            if (uniq.size() > EK_PART_MAX_GROUPS) { host = true; break; }
-        }
-        if (!host) {
-            /* (2) one compaction of the index sequence per distinct value */
-            Handle idx(ek_trace_append(EK_UINT32, EK_OP_INDEX, 0, 0, 0, 0));
-            if (!idx || ek_var_set_size(idx.h, n, 0) == 0 || ek_eval_var(idx.h) != 0) return -1;
-            perm_h = (uint32_t **) malloc(sizeof(uint32_t *) * uniq.size());
-            for (size_t k = 0; k < uniq.size(); ++k) {
-                Handle lv = lit64(uniq[k]);
-                Handle eq(ek_trace_append(EK_BOOL, EK_OP_EQ, kv.h, lv.h, 0, 0));
-                void *out = nullptr; size_t cnt = 0;
-                if (!lv || !eq || ek_eval_var(eq.h) != 0 ||
-                    ek_compress(EK_UINT32, n, ek_var_ptr(idx.h), (const uint8_t *) ek_var_ptr(eq.h), &out, &cnt) != 0) {
-                    for (size_t j = 0; j < k; ++j) ek_free(perm_h[j]);
-                    free(perm_h);
-                    return -1;
-                }
-                perm_h[k] = (uint32_t *) out;
-                cnts.push_back((uint32_t) cnt);
-            }
-            ek_cuda_check(cudaStreamSynchronize(ctx.stream));
-        }
-    }
-    if (host) {
-        uniq.clear(); cnts.clear();
-        if (partition_host_sort(ctx, n, keys, uniq, cnts, perm_h) != 0) return -1;
-    }
-    /* outputs with the reference's ownership: pinned-host unique / counts (counts[0] = number of groups,
-       horiz.cu:83-121), malloc'd array of device permutation pointers */
-    const size_t K = uniq.size();
-    uint32_t *counts_h = (uint32_t *) ek_host_malloc(sizeof(uint32_t) * (K + 1));
-    void **unique_h = (void **) ek_host_malloc(sizeof(void *) * std::max<size_t>(K, 1));
-    counts_h[0] = (uint32_t) K;
-    for (size_t k = 0; k < K; ++k) { counts_h[k + 1] = cnts[k]; unique_h[k] = (void *) (uintptr_t) uniq[k]; }
-    *unique_out = unique_h; *counts_out = counts_h; *perm_out = perm_h;
-    return 0;
 }
 
 } /* extern "C" */

@@ -379,7 +379,8 @@ struct CUDAArray : ArrayBase<value_t<Value>, CUDAArray<Value>> {
 
     /// Virtual-call dispatch support (cuda.h:814-843): (instance pointer, indices that refer to it), pointers ascending,
     /// indices ascending; cached per array like the reference's.
-    /// (ek_partition: host-side stable sort by default, device composition with EK_PARTITION_DEVICE=1, see ek_scan.cu.)
+    /// (ek_partition: hash + radix grouping on the device up to 65 536 distinct pointers, host-side stable sort above,
+    /// see ek_partition.cu.)
     template <typename T = Value, enable_if_t<std::is_pointer_v<T> || std::is_same_v<T, uintptr_t>> = 0>
     std::vector<std::pair<Value, CUDAArray<uint32_t>>> partition_() const {
         using Groups = std::vector<std::pair<Value, CUDAArray<uint32_t>>>;

@@ -240,6 +240,7 @@ typedef struct ek_stats {
     float    last_kernel_ms;    /* device time of the most recent timed launch (timing mode only) */
     float    total_kernel_ms;   /* sum of device times since reset (timing mode only)     */
     uint64_t fast_launches;     /* ... sweeps that ran on the 32-bit fast kernel (ek_sweep_fast.cu) */
+    uint64_t partition_device;  /* ek_partition calls grouped on the device (the rest fell back to the host sort) */
 } ek_stats;
 /* ------------------------------------------------------------------ multi-GPU (SURVEY 8e; no counterpart in the reference)
  * One rank (process) per GPU, element-range sharding, ONE all-reduce of the size-1 results per step (the local hsum is
