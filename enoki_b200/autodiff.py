@@ -103,7 +103,7 @@ class FloatD:
         from . import rcp
         o = FloatD._c(o)
         rb = rcp(o.value)                                  # autodiff.h:258-272
-        return FloatD._node("div", self.value / o.value, [self, o], [rb, -self.value * rb * rb])
+        return FloatD._node("div", self.value / o.value, [self, o], [rb, -self.value * (rb * rb)])
 
     def __rtruediv__(self, o):
         return FloatD._c(o) / self
@@ -124,7 +124,12 @@ def _unary(label, f, dfdx):
 
 
 def _build():
-    from . import sin as _sin, cos as _cos, exp as _exp, log as _log, sqrt as _sqrt, rcp as _rcp, Float32, select
+    from . import sin as _sin, cos as _cos, exp as _exp, log as _log, sqrt as _sqrt, rcp as _rcp, Float32, UInt32, reinterpret
+
+    def _sign(a):
+        # sign(a) = (sign_mask & a) | 1.0 (array_router.h:372): -1 at -0.0 and at NaNs with the sign bit set
+        return reinterpret(Float32, (reinterpret(UInt32, a) & 0x80000000) | 0x3f800000)
+
     g = {}
     g["sin"] = _unary("sin", _sin, lambda a, r: _cos(a))
     g["cos"] = _unary("cos", _cos, lambda a, r: -_sin(a))
@@ -132,8 +137,7 @@ def _build():
     g["log"] = _unary("log", _log, lambda a, r: _rcp(a))
     g["sqrt"] = _unary("sqrt", _sqrt, lambda a, r: Float32(0.5) / r)       # autodiff.h:353-364
     g["rcp"] = _unary("rcp", _rcp, lambda a, r: -(r * r))                  # autodiff.h:379-390
-    g["abs"] = _unary("abs", lambda a: abs(a),
-                      lambda a, r: select(a >= 0.0, Float32(1.0), Float32(-1.0)))   # sign(a), autodiff.h:341-351
+    g["abs"] = _unary("abs", lambda a: abs(a), lambda a, r: _sign(a))      # autodiff.h:341-351
     return g
 
 

@@ -395,6 +395,7 @@ int backward_impl(Tape &T, bool free_graph) {
     for (size_t i = 0; i < S; ++i) { pos_of[sched[i] - id_base] = (uint32_t) i; sn[i].n = node(T, sched[i]); }
     uint32_t max_level = 0;
     bool need_eval = false;
+    const bool any_dirty = !ctx.dirty.empty();
     size_t total_terms = 0;
     /* out-edge lists in CSR form (no per-node allocations): count, prefix-sum, fill */
     std::vector<uint32_t> out_start(S + 1, 0);
@@ -417,9 +418,12 @@ int backward_impl(Tape &T, bool free_graph) {
             max_level = std::max(max_level, sn[p].level);
             out_items[cursor[p]++] = OutEdge((uint32_t) i, &e);
             if (!e.special) {
+                /* a dirty weight has pending side effects (the zeroing scatter of a scatter_combine edge):
+                   the kernel must not read its buffer before they ran.  The flag sits on another cache line
+                   than `data`, so it is only read while some variable is dirty at all. */
                 const EkVariable &w = ctx.vars[e.weight];
                 uint64_t bits;
-                if (w.data == nullptr && !var_imm(e.weight, bits)) need_eval = true;
+                if ((w.data == nullptr && !var_imm(e.weight, bits)) || (any_dirty && w.dirty)) need_eval = true;
             }
         }
     }
@@ -692,9 +696,22 @@ int forward_impl(Tape &T, bool free_graph) {
                             ek_var_mark_side_effect(h);
                             ek_var_mark_dirty(t.grad);
                         } break;
-                        default:
-                            ek_set_error("forward(): psum/reverse edges are not implemented yet");
-                            return -1;
+                        case SP_REVERSE:           /* autodiff.cpp:430-440 */
+                        case SP_PSUM: {            /* autodiff.cpp:480-490 */
+                            if (ek_eval_var(g) != 0) return -1;
+                            size_t n = ek_var_size(g), es = ek_type_size(T.vt);
+                            void *p;
+                            if (sp.kind == SP_PSUM) {
+                                p = ek_psum(T.vt, n, ek_var_ptr(g));
+                                if (!p) return -1;
+                            } else {
+                                p = ek_malloc(n * es);
+                                ek_reverse(p, ek_var_ptr(g), es, n);
+                            }
+                            uint32_t r = ek_var_register(T.vt, n, p, 1);
+                            if (!t.grad) set_grad(t, r);
+                            else { uint32_t a = v_op(T.vt, EK_OP_ADD, t.grad, r); ek_dec_ref_ext(r); if (!a) return -1; set_grad(t, a); }
+                        } break;
                     }
                 }
             }

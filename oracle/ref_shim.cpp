@@ -373,15 +373,16 @@ void ref_morton2_decode(const uint32_t *m, uint32_t *x_, uint32_t *y_, size_t n)
  *   n_nodes nodes; node i has size node_size[i]; nodes with no in-edges are
  *   leaves.  Edge e: src[e] -> dst[e] with weight array weights + woff[e]
  *   of length wsize[e] (1 or node size).  Edges must be listed grouped by
- *   dst in ascending dst order (tape creation order).  backward() from
- *   `root` (1-based position in node list), seeds grad 1, and copies the
- *   gradient of every node listed in want[] into grads_out (concatenated).
+ *   dst in ascending dst order (tape creation order).  backward() (or
+ *   forward()) from `root` (1-based position in node list), seeds grad 1,
+ *   and copies the gradient of every node listed in want[] into grads_out
+ *   (concatenated; an empty gradient reads as zeros).
  */
-int ref_tape_backward(uint32_t n_nodes, const uint32_t *node_size,
-                      uint32_t n_edges, const uint32_t *src, const uint32_t *dst,
-                      const float *weights, const uint64_t *woff, const uint32_t *wsize,
-                      uint32_t root, uint32_t n_want, const uint32_t *want,
-                      float *grads_out, int free_graph) {
+static int ref_tape_sweep(bool forward, uint32_t n_nodes, const uint32_t *node_size,
+                          uint32_t n_edges, const uint32_t *src, const uint32_t *dst,
+                          const float *weights, const uint64_t *woff, const uint32_t *wsize,
+                          uint32_t root, uint32_t n_want, const uint32_t *want,
+                          float *grads_out, int free_graph) {
     try {
         TapeX *tape = TapeX::get();
         tape->set_graph_simplification(false);
@@ -391,7 +392,8 @@ int ref_tape_backward(uint32_t n_nodes, const uint32_t *node_size,
             if (e < n_edges && dst[e] == i) {
                 ids[i] = tape->append_node(node_size[i - 1], "n");
                 while (e < n_edges && dst[e] == i) {
-                    FloatX w = FloatX::copy(weights + woff[e], wsize[e]);
+                    /* size-1 operands broadcast their whole first packet (dynamic.h:302-318): fill every lane */
+                    FloatX w = wsize[e] == 1 ? full<FloatX>(weights[woff[e]], 1) : FloatX::copy(weights + woff[e], wsize[e]);
                     tape->append_edge(ids[src[e]], ids[i], w);
                     ++e;
                 }
@@ -400,7 +402,8 @@ int ref_tape_backward(uint32_t n_nodes, const uint32_t *node_size,
             }
         }
         if (e != n_edges) return -2;
-        tape->backward(ids[root], free_graph != 0);
+        if (forward) tape->forward(ids[root], free_graph != 0);
+        else tape->backward(ids[root], free_graph != 0);
         size_t off = 0;
         for (uint32_t k = 0; k < n_want; ++k) {
             const FloatX &g = tape->gradient(ids[want[k]]);
@@ -415,9 +418,27 @@ int ref_tape_backward(uint32_t n_nodes, const uint32_t *node_size,
             tape->dec_ref_ext(ids[i]);
         return 0;
     } catch (const std::exception &ex) {
-        fprintf(stderr, "ref_tape_backward: %s\n", ex.what());
+        fprintf(stderr, "ref_tape_%s: %s\n", forward ? "forward" : "backward", ex.what());
         return -1;
     }
+}
+
+int ref_tape_backward(uint32_t n_nodes, const uint32_t *node_size,
+                      uint32_t n_edges, const uint32_t *src, const uint32_t *dst,
+                      const float *weights, const uint64_t *woff, const uint32_t *wsize,
+                      uint32_t root, uint32_t n_want, const uint32_t *want,
+                      float *grads_out, int free_graph) {
+    return ref_tape_sweep(false, n_nodes, node_size, n_edges, src, dst, weights, woff, wsize,
+                          root, n_want, want, grads_out, free_graph);
+}
+
+int ref_tape_forward(uint32_t n_nodes, const uint32_t *node_size,
+                     uint32_t n_edges, const uint32_t *src, const uint32_t *dst,
+                     const float *weights, const uint64_t *woff, const uint32_t *wsize,
+                     uint32_t root, uint32_t n_want, const uint32_t *want,
+                     float *grads_out, int free_graph) {
+    return ref_tape_sweep(true, n_nodes, node_size, n_edges, src, dst, weights, woff, wsize,
+                          root, n_want, want, grads_out, free_graph);
 }
 
 /* Public-API autodiff checks (tests/autodiff.cpp shapes): d/dx of a small expression */

@@ -95,6 +95,7 @@ def main():
     np.savez_compressed(os.path.join(HERE, "ad_expr.npz"), **d)
     ref_math()
     ref_tape()
+    ref_tape_sweep()
     shim_plan()
     print("golden vectors written to", HERE)
 
@@ -125,6 +126,33 @@ def ref_tape(w=64):
                                P(g["weights"]), P(g["woff"]), P(g["wsize"]), int(g["root"]), len(g["want"]), P(g["want"]),
                                P(grads), 1) == 0
     np.savez_compressed(os.path.join(HERE, "ref_tape.npz"), grads=grads, **g)
+
+
+def ref_tape_sweep(n_graphs=48):
+    """The reference tape's backward() and forward() from one seed on random general graphs (ref_tape_sweep.npz):
+    tests/test_gpu_tape_graphs.random_graph with size-1 nodes joined to wide ones or not, with and without
+    free_graph.  Every node's gradient is stored; an empty one reads as zeros."""
+    import sys
+    sys.path.insert(0, os.path.dirname(HERE))
+    from test_gpu_tape_graphs import random_graph
+    d = {}
+    for k in range(n_graphs):
+        rng = np.random.default_rng([21, k])
+        forward, free_graph, mixed = k & 1, (k >> 1) & 1, (k >> 2) & 1
+        g = random_graph(rng, 24, np.float32, mixed=bool(mixed), widths=(3, 4, 5, 17, 33, 67))
+        n = len(g["node_size"])
+        outs = np.bincount(g["src"].astype(np.int64), minlength=n + 1)
+        root = int(np.argmax(outs)) if forward else n
+        want = np.arange(1, n + 1, dtype=np.uint32)
+        grads = np.zeros(int(g["node_size"].astype(np.int64).sum()), np.float32)
+        fn = R.ref_tape_forward if forward else R.ref_tape_backward
+        assert fn(n, P(g["node_size"]), len(g["src"]), P(g["src"]), P(g["dst"]), P(g["weights"]), P(g["woff"]),
+                  P(g["wsize"]), root, n, P(want), P(grads), free_graph) == 0
+        for key in ("node_size", "src", "dst", "weights", "woff", "wsize"):
+            d[f"{k}_{key}"] = g[key]
+        d[f"{k}_mode"] = np.array([forward, free_graph, root], np.uint32)
+        d[f"{k}_grads"] = grads
+    np.savez_compressed(os.path.join(HERE, "ref_tape_sweep.npz"), n_graphs=n_graphs, **d)
 
 
 def shim_plan():

@@ -160,6 +160,32 @@ def test_oracle_vs_reference_tape(oracle, ref, P):
     assert (a.view(np.uint32) == b.view(np.uint32)).all()
 
 
+def test_oracle_tape_sweep_vs_reference(oracle, ref, P):
+    """or_tape_sweep_f32 against the reference's own Tape::backward / Tape::forward on 48 random general graphs
+    (tests/golden/ref_tape_sweep.npz): widths mixed with size-1 nodes (hsum and broadcast), skip-level and
+    duplicated edges, exact zeros next to inf / NaN, both modes, with and without free_graph.  Where oracle/_ref
+    carries a reference library built from this repository's ref_shim.cpp (it has ref_tape_forward), that library
+    is also checked to still compute exactly the stored gradients."""
+    from test_gpu_tape_graphs import assert_same, oracle_sweep
+    gold = np.load(os.path.join(GOLD, "ref_tape_sweep.npz"))
+    live = ref is not None and hasattr(ref, "ref_tape_forward")
+    for k in range(int(gold["n_graphs"])):
+        g = {key: gold[f"{k}_{key}"] for key in ("node_size", "src", "dst", "weights", "woff", "wsize")}
+        forward, free_graph, root = (int(v) for v in gold[f"{k}_mode"])
+        stored = gold[f"{k}_grads"]
+        a, rc = oracle_sweep(oracle, g, [(root, 1.0)], forward, free_graph)
+        assert rc == 0
+        assert_same(a, stored, f"oracle, graph {k}")
+        if live:
+            n = len(g["node_size"])
+            want = np.arange(1, n + 1, dtype=np.uint32)
+            b = np.zeros_like(stored)
+            fn = ref.ref_tape_forward if forward else ref.ref_tape_backward
+            assert fn(n, P(g["node_size"]), len(g["src"]), P(g["src"]), P(g["dst"]), P(g["weights"]), P(g["woff"]),
+                      P(g["wsize"]), root, n, P(want), P(b), free_graph) == 0
+            assert_same(b, stored, f"reference, graph {k}")
+
+
 def test_histogram_known_answer(oracle, P):
     """tests/histogram.cpp:68-73: 16 Mi PCG32 samples -> erfinv -> 31 bins; bins[1]==2558, bins[2]==6380,
     743 +- 3 samples out of range.  erfinv is not restated in the oracle (it is traced op-by-op on the
