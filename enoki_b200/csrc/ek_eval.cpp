@@ -1348,27 +1348,31 @@ bool lower_fast(const std::vector<EkInstr> &in, const Assembled &a, const Config
     return true;
 }
 
+/* kernel configurations, tried in order (V, T, stages, CTAs per SM) */
+struct Cand { int V; uint32_t T; uint32_t stages; uint32_t want_ctas; };
+/* the 32-bit fast kernel: V = 16, one TMA stage (the other CTAs of the SM hide the load) */
+const Cand fast_cands[] = { { 16, 256, 1, 2 }, { 16, 128, 1, 4 }, { 16, 128, 1, 3 }, { 16, 128, 1, 2 }, { 16, 256, 1, 1 }, { 16, 128, 1, 1 } };
+const Cand wide_cands[] = {
+    /* the general kernel: single-buffered staging with more resident CTAs first, double buffering after: the
+       other CTAs of the SM hide the TMA latency and 16 warps hide the interpreter's dependent-issue latency */
+    { 8, 256, 1, 4 }, { 8, 256, 1, 3 }, { 8, 256, 2, 2 }, { 8, 256, 1, 2 }, { 8, 256, 2, 1 }, { 8, 256, 1, 1 },
+    /* (no { 8, 128, 1, 2 }: a program that { 8, 256, 1, 1 } rejects needs more than half of an SM's shared memory at
+       T = 128, so two such CTAs never fit) */
+    { 8, 128, 2, 1 }, { 8, 128, 1, 1 },
+    { 4, 128, 2, 1 }, { 4, 64, 2, 1 }, { 4, 32, 2, 1 } };
+/* tiny sweeps (incl. the size-1 scalar groups): one small CTA */
+const Cand small_cands[] = { { 4, 32, 2, 1 }, { 4, 128, 2, 1 }, { 8, 256, 2, 1 } };
+
 bool choose_config(const EkContext &ctx, const Assembled &a, size_t n, Config &cfg, std::string &err) {
     size_t n_uni = a.lits.size() + a.argw.size() + 2 * a.scalars.size();
     size_t budget = ctx.smem_optin;                 /* per CTA (227 KB) */
     size_t per_sm = 228 * 1024 - 1024;              /* per SM, minus the 1 KB per-CTA reservation */
-    struct Cand { int V; uint32_t T; uint32_t stages; uint32_t want_ctas; };
-    /* the 32-bit fast kernel: V = 16, one TMA stage (the other CTAs of the SM hide the load) */
-    static const Cand fast_cands[] = { { 16, 256, 1, 2 }, { 16, 128, 1, 4 }, { 16, 128, 1, 3 }, { 16, 128, 1, 2 }, { 16, 256, 1, 1 }, { 16, 128, 1, 1 } };
-    static const Cand cands[] = {
-        /* the general kernel: single-buffered staging with more resident CTAs first, double buffering after: the
-           other CTAs of the SM hide the TMA latency and 16 warps hide the interpreter's dependent-issue latency */
-        { 8, 256, 1, 4 }, { 8, 256, 1, 3 }, { 8, 256, 2, 2 }, { 8, 256, 1, 2 }, { 8, 256, 2, 1 }, { 8, 256, 1, 1 },
-        { 8, 128, 1, 2 }, { 8, 128, 2, 1 }, { 8, 128, 1, 1 },
-        { 4, 128, 2, 1 }, { 4, 64, 2, 1 }, { 4, 32, 2, 1 } };
     const bool fast_ok = ctx.fast_mode != 0 && !a.has64 && a.fast_ok && a.fast_len <= EK_INLINE_PROG;
     cfg.fast = false;
     if (n <= 4096) {
-        /* tiny sweeps (incl. the size-1 scalar groups): one small CTA */
-        static const Cand small[] = { { 4, 32, 2, 1 }, { 4, 128, 2, 1 }, { 8, 256, 2, 1 } };
         uint32_t pick = n <= 128 ? 0 : n <= 512 ? 1 : 2;
         for (uint32_t k = pick; k < 3; ++k) {
-            cfg.V = small[k].V; cfg.T = small[k].T; cfg.stages = 2; cfg.ctas_per_sm = 1;
+            cfg.V = small_cands[k].V; cfg.T = small_cands[k].T; cfg.stages = 2; cfg.ctas_per_sm = 1;
             if (smem_layout(a, cfg, n_uni) <= budget) return true;
         }
     }
@@ -1387,7 +1391,7 @@ bool choose_config(const EkContext &ctx, const Assembled &a, size_t n, Config &c
         }
         cfg.fast = false;
     }
-    for (const Cand &c : cands) {
+    for (const Cand &c : wide_cands) {
         cfg.V = c.V; cfg.T = c.T; cfg.stages = a.n_in_units ? c.stages : 2; cfg.ctas_per_sm = c.want_ctas;
         size_t need = smem_layout(a, cfg, n_uni);
         if (need > budget) continue;
@@ -1593,6 +1597,15 @@ static int eval_impl(bool dry, std::string *dump, bool json = false) {
                 oss << "],\"outputs\":[";
                 for (size_t i = 0; i < a.outputs.size(); ++i) oss << (i ? "," : "") << "[" << a.outputs[i].var << "," << a.outputs[i].argw << "," << a.outputs[i].bytes << "," << (int) ctx.vars[a.outputs[i].var].type << "]";
                 oss << "]";
+                {   /* the configuration the launcher picks for this sweep as it stands */
+                    Config lcfg; std::string lerr;
+                    if (choose_config(ctx, a, l.first->size, lcfg, lerr))
+                        oss << ",\"config\":{\"fast\":" << (lcfg.fast ? 1 : 0) << ",\"V\":" << lcfg.V << ",\"T\":" << lcfg.T
+                            << ",\"stages\":" << lcfg.stages << ",\"ctas_per_sm\":" << lcfg.ctas_per_sm << ",\"smem\":" << lcfg.smem
+                            << ",\"prog_in_smem\":" << (lcfg.prog_in_smem ? 1 : 0)
+                            << ",\"inline_prog\":" << (a.init.size() + a.body.size() + a.fini.size() <= EK_INLINE_PROG ? 1 : 0)
+                            << ",\"inline_lit\":" << (a.lits.size() <= EK_MAX_LIT_INLINE ? 1 : 0) << "}";
+                }
                 /* the program as the 32-bit fast kernel would receive it (lower_fast), when that is the kernel the
                    launcher would pick for this sweep */
                 Config fcfg; std::string ferr;
@@ -1622,7 +1635,18 @@ static int eval_impl(bool dry, std::string *dump, bool json = false) {
                 }
                 oss << "}";
             }
-            oss << "],\"fops\":[";
+            oss << "],\"configs\":{";
+            {   /* the candidate lists of choose_config, in the order it tries them */
+                auto cl = [&](const char *name, const Cand *c, size_t k, bool last) {
+                    oss << "\"" << name << "\":[";
+                    for (size_t i = 0; i < k; ++i) oss << (i ? "," : "") << "[" << c[i].V << "," << c[i].T << "," << c[i].stages << "," << c[i].want_ctas << "]";
+                    oss << "]" << (last ? "" : ",");
+                };
+                cl("small", small_cands, sizeof(small_cands) / sizeof(Cand), false);
+                cl("fast", fast_cands, sizeof(fast_cands) / sizeof(Cand), false);
+                cl("wide", wide_cands, sizeof(wide_cands) / sizeof(Cand), true);
+            }
+            oss << "},\"fops\":[";
             {
                 static const char *fnames[] = { "NOP",
 #define X(n) #n, #n "_U",
