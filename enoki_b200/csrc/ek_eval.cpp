@@ -24,7 +24,6 @@ static_assert(sizeof(EkSweepArgs) <= 32000, "EkSweepArgs must fit the 32 KB kern
 #include <cstdlib>
 #include <cstring>
 #include <algorithm>
-#include <functional>
 #include <sstream>
 #include <unordered_set>
 #include <memory>
@@ -217,7 +216,6 @@ struct Assembler {
     EkContext &ctx;
     const Group &g;
     const std::unordered_set<uint32_t> &forced;
-    bool dry;
     Assembled out;
 
     std::unordered_map<uint32_t, Loc> loc;
@@ -235,8 +233,8 @@ struct Assembler {
     uint32_t acc_var = 0;
     uint32_t cur_e = 0;
 
-    Assembler(EkContext &c, const Group &gr, const std::unordered_set<uint32_t> &f, bool d)
-        : ctx(c), g(gr), forced(f), dry(d) {}
+    Assembler(EkContext &c, const Group &gr, const std::unordered_set<uint32_t> &f)
+        : ctx(c), g(gr), forced(f) {}
 
     const EkVariable &var(uint32_t i) const { return ctx.vars[i]; }
     bool wide() const { return g.size > 1; }
@@ -1348,6 +1346,45 @@ bool lower_fast(const std::vector<EkInstr> &in, const Assembled &a, const Config
     return true;
 }
 
+/* a program as one kernel reads it */
+struct Program {
+    std::vector<EkInstr> init, body, fini;
+    size_t size() const { return init.size() + body.size() + fini.size(); }
+};
+
+/* lower_fast on all three sections (the body with its release NOP) */
+bool lower_fast_all(const Assembled &a, const Config *cfg, Program &p) {
+    return lower_fast(a.init, a, cfg, p.init) && lower_fast(a.body, a, cfg, p.body, a.release_at) && lower_fast(a.fini, a, cfg, p.fini);
+}
+
+/* the program the kernel of `cfg` receives: for the general kernels the operand codes become (byte offset >> 4) in
+   this configuration's shared-memory layout; for the fast kernel, the lowered form */
+bool kernel_program(const Assembled &a, const Config &cfg, Program &p) {
+    if (cfg.fast) return lower_fast_all(a, &cfg, p);
+    const uint32_t slot_bytes = cfg.T * cfg.V * 4u;
+    auto patch = [&](uint16_t code) -> uint16_t {
+        if (code == EK_OPND_NONE || (code & EK_OPND_UNI)) return code;      /* uniform index == offset >> 4 */
+        if (code & EK_OPND_STAGED) return (uint16_t) (EK_OPND_STAGED | (((code & 0x3fffu) * slot_bytes) >> 4));
+        return (uint16_t) ((cfg.off_slots + (uint32_t) code * slot_bytes) >> 4);
+    };
+    auto patch_all = [&](const std::vector<EkInstr> &from, std::vector<EkInstr> &v) {
+        v = from;
+        for (EkInstr &in : v) {
+            in.b = patch(in.b); in.c = patch(in.c);
+            if (in.flags & EKF_HAS_A) in.a = patch(in.a);
+            if ((in.flags & (EKF_ST | EKF_RACC)) || in.op == DOP_RACC) in.dst = patch(in.dst);
+        }
+    };
+    patch_all(a.init, p.init); patch_all(a.body, p.body); patch_all(a.fini, p.fini);
+    return true;
+}
+
+/* the argument words the kernel of `cfg` receives, pointer words not yet filled in */
+void argument_words(const Assembled &a, const Config &cfg, uint32_t *argw) {
+    if (!a.argw.empty()) memcpy(argw, a.argw.data(), a.argw.size() * 4);
+    layout_extra(a, cfg, argw);
+}
+
 /* kernel configurations, tried in order (V, T, stages, CTAs per SM) */
 struct Cand { int V; uint32_t T; uint32_t stages; uint32_t want_ctas; };
 /* the 32-bit fast kernel: V = 16, one TMA stage (the other CTAs of the SM hide the load) */
@@ -1412,18 +1449,19 @@ uint64_t fnv1a(const uint8_t *p, size_t n) {
 /* device copies of programs / literal pools that do not fit the kernel parameters (rare: > 448 instructions or > 128
    literal words).  Keyed on exactly what is uploaded; bounded: the cache is emptied when it reaches 256 entries (the
    stream is synchronised first, so no launch still reads the freed buffers). */
-void lookup_program(EkContext &ctx, const Assembled &a, bool need_prog, bool need_lit, const EkInstr *&d_prog, const uint32_t *&d_lit) {
+void lookup_program(EkContext &ctx, const Program &prog, const std::vector<uint32_t> &lits, bool need_prog, bool need_lit,
+                    const EkInstr *&d_prog, const uint32_t *&d_lit) {
     std::vector<uint8_t> key;
     auto append = [&](const void *p, size_t n) { const uint8_t *b = (const uint8_t *) p; key.insert(key.end(), b, b + n); };
-    uint32_t hdr[4] = { need_prog ? (uint32_t) a.init.size() : 0u, need_prog ? (uint32_t) a.body.size() : 0u, need_prog ? (uint32_t) a.fini.size() : 0u,
-                        need_lit ? (uint32_t) a.lits.size() : 0u };
+    uint32_t hdr[4] = { need_prog ? (uint32_t) prog.init.size() : 0u, need_prog ? (uint32_t) prog.body.size() : 0u,
+                        need_prog ? (uint32_t) prog.fini.size() : 0u, need_lit ? (uint32_t) lits.size() : 0u };
     append(hdr, sizeof(hdr));
     if (need_prog) {
-        append(a.init.data(), a.init.size() * sizeof(EkInstr));
-        append(a.body.data(), a.body.size() * sizeof(EkInstr));
-        append(a.fini.data(), a.fini.size() * sizeof(EkInstr));
+        append(prog.init.data(), prog.init.size() * sizeof(EkInstr));
+        append(prog.body.data(), prog.body.size() * sizeof(EkInstr));
+        append(prog.fini.data(), prog.fini.size() * sizeof(EkInstr));
     }
-    if (need_lit) append(a.lits.data(), a.lits.size() * 4);
+    if (need_lit) append(lits.data(), lits.size() * 4);
     uint64_t h = fnv1a(key.data(), key.size());
     {
         auto it = ctx.programs.find(h);
@@ -1442,16 +1480,16 @@ void lookup_program(EkContext &ctx, const Assembled &a, bool need_prog, bool nee
     e.d_prog = nullptr; e.d_lit = nullptr;
     if (need_prog) {
         std::vector<EkInstr> all;
-        all.insert(all.end(), a.init.begin(), a.init.end());
-        all.insert(all.end(), a.body.begin(), a.body.end());
-        all.insert(all.end(), a.fini.begin(), a.fini.end());
+        all.insert(all.end(), prog.init.begin(), prog.init.end());
+        all.insert(all.end(), prog.body.begin(), prog.body.end());
+        all.insert(all.end(), prog.fini.begin(), prog.fini.end());
         ek_cuda_check(cudaMalloc(&e.d_prog, std::max<size_t>(all.size(), 1) * sizeof(EkInstr)));
         /* synchronous copies from pageable memory: only on a cache miss */
         if (!all.empty()) ek_cuda_check(cudaMemcpy(e.d_prog, all.data(), all.size() * sizeof(EkInstr), cudaMemcpyHostToDevice));
     }
     if (need_lit) {
-        ek_cuda_check(cudaMalloc(&e.d_lit, std::max<size_t>(a.lits.size(), 1) * 4));
-        if (!a.lits.empty()) ek_cuda_check(cudaMemcpy(e.d_lit, a.lits.data(), a.lits.size() * 4, cudaMemcpyHostToDevice));
+        ek_cuda_check(cudaMalloc(&e.d_lit, std::max<size_t>(lits.size(), 1) * 4));
+        if (!lits.empty()) ek_cuda_check(cudaMemcpy(e.d_lit, lits.data(), lits.size() * 4, cudaMemcpyHostToDevice));
     }
     d_prog = e.d_prog; d_lit = e.d_lit;
     ctx.programs[h].push_back(std::move(e));
@@ -1492,60 +1530,63 @@ void dump_program(std::ostream &os, const Assembled &a, const Group &g) {
     sec("init", a.init); sec("body", a.body); sec("fini", a.fini);
 }
 
-} // namespace
+/* ------------------------------------------------------------------ the sweeps of one eval */
+/* one kernel launch: a group, its assembled program (operand codes still symbolic) and the configuration it runs with */
+struct Sweep { Group *g; Assembled a; Config cfg; };
 
-/* ------------------------------------------------------------------ eval */
-static int eval_impl(bool dry, std::string *dump, bool json = false) {
-    EkContext &ctx = ek_ctx();
-
-    if (!dry) for (auto cb : ctx.callbacks) cb.first(cb.second);         /* jit.cu:1421-1422 */
-    if (ctx.live.empty()) {
-        if (!dry) { for (uint32_t idx : ctx.dirty) if (idx < ctx.vars.size()) ctx.vars[idx].dirty = false; ctx.dirty.clear(); }
-        return 0;
-    }
-    if (!dry && ek_init() != 0) return -1;
-
-    Planner plan(ctx);
-    std::vector<uint32_t> kept_literals;
-    /* Roots are planned in CREATION order: the reference walks a std::set of monotonically increasing ids
-       (jit.cu:1385-1416), so of two scatters into the same target the one recorded later runs later and wins, a
-       scatter recorded after a gather from the same array comes after it, and so on.  Handles are recycled here, so
-       the order is the per-variable sequence number, not the handle. */
-    std::vector<uint32_t> work(ctx.live.begin(), ctx.live.end());
-    std::sort(work.begin(), work.end(), [&](uint32_t a, uint32_t b) { return ctx.vars[a].seq > ctx.vars[b].seq; });
-    std::vector<uint32_t> roots = work;
-    while (!work.empty()) {                              /* (pop_back: oldest first) */
-        uint32_t idx = work.back(); work.pop_back();
-        const EkVariable &v = ctx.vars[idx];
-        if (!v.used) continue;
-        if (v.data != nullptr && !v.side_effect) continue;
-        /* literals are immediates: they are only given storage on demand (ek_eval_var) */
-        if (v.op == EK_OP_LITERAL) { kept_literals.push_back(idx); continue; }
-        plan.add_root(idx, work);
-    }
-
-    /* assemble every group first so that user errors leave the trace untouched */
+/* what ek_eval() launches for the live set, in launch order, together with the groups the sweeps point into */
+struct Schedule {
+    Planner plan;
     std::vector<std::unique_ptr<Group>> split_groups;
-    std::vector<std::pair<Group *, Assembled>> launches;
-    std::string asm_error;
+    std::vector<Sweep> sweeps;
+    std::vector<uint32_t> kept_literals;      /* live literals: no sweep computes them, they stay live */
+
+    explicit Schedule(EkContext &ctx) : plan(ctx) {}
+
+    /* assemble every group before anything is launched, so that user errors leave the trace untouched */
+    bool build() {
+        EkContext &ctx = plan.ctx;
+        /* Roots are planned in CREATION order: the reference walks a std::set of monotonically increasing ids
+           (jit.cu:1385-1416), so of two scatters into the same target the one recorded later runs later and wins, a
+           scatter recorded after a gather from the same array comes after it, and so on.  Handles are recycled here, so
+           the order is the per-variable sequence number, not the handle. */
+        std::vector<uint32_t> work(ctx.live.begin(), ctx.live.end());
+        std::sort(work.begin(), work.end(), [&](uint32_t a, uint32_t b) { return ctx.vars[a].seq > ctx.vars[b].seq; });
+        while (!work.empty()) {                              /* (pop_back: oldest first) */
+            uint32_t idx = work.back(); work.pop_back();
+            const EkVariable &v = ctx.vars[idx];
+            if (!v.used) continue;
+            if (v.data != nullptr && !v.side_effect) continue;
+            /* literals are immediates: they are only given storage on demand (ek_eval_var) */
+            if (v.op == EK_OP_LITERAL) { kept_literals.push_back(idx); continue; }
+            plan.add_root(idx, work);
+        }
+        for (auto &kv : plan.groups)                         /* ordered by (phase asc, size asc) */
+            if (!assemble(kv.second)) return false;
+        /* within a phase launch the largest size first (jit.cu:1450) */
+        std::stable_sort(sweeps.begin(), sweeps.end(), [](const Sweep &a, const Sweep &b) {
+            if (a.g->phase != b.g->phase) return a.g->phase < b.g->phase;
+            return a.g->size > b.g->size; });
+        return true;
+    }
+
     /* assemble `g`; when a per-kernel limit is hit (slots, inputs, arguments ...) split its roots in
        two and retry -- shared sub-expressions are then recomputed, exactly as the reference does
        across kernels of different sizes */
-    std::function<bool(Group &)> assemble_group = [&](Group &g) -> bool {
+    bool assemble(Group &g) {
         if (g.sched.empty()) return true;
-        if (g.size > 0xffffffffull) { asm_error = "arrays with more than 2^32-1 entries are not supported (jit.cu:1066,1090)"; return false; }
-        Assembler as(ctx, g, plan.forced, dry);
+        if (g.size > 0xffffffffull) { ek_set_error("ek_eval(): arrays with more than 2^32-1 entries are not supported (jit.cu:1066,1090)"); return false; }
+        Assembler as(plan.ctx, g, plan.forced);
         bool ok = as.run();
         if (ok && !as.out.has64) {
-            std::vector<EkInstr> lowered;
-            as.out.fast_ok = lower_fast(as.out.init, as.out, nullptr, lowered) && lower_fast(as.out.body, as.out, nullptr, lowered, as.out.release_at) &&
-                             lower_fast(as.out.fini, as.out, nullptr, lowered);
+            Program lowered;
+            as.out.fast_ok = lower_fast_all(as.out, nullptr, lowered);
             as.out.fast_len = (uint32_t) lowered.size();
         }
         Config cfg; std::string cerr;
-        if (ok && !choose_config(ctx, as.out, g.size, cfg, cerr)) { ok = false; as.out.error = cerr; as.out.resource_error = true; }
-        if (ok) { launches.emplace_back(&g, std::move(as.out)); return true; }
-        if (!as.out.resource_error || g.roots.size() < 2) { asm_error = as.out.error; return false; }
+        if (ok && !choose_config(plan.ctx, as.out, g.size, cfg, cerr)) { ok = false; as.out.error = cerr; as.out.resource_error = true; }
+        if (ok) { sweeps.push_back({ &g, std::move(as.out), cfg }); return true; }
+        if (!as.out.resource_error || g.roots.size() < 2) { ek_set_error("ek_eval(): " + as.out.error); return false; }
         size_t half = g.roots.size() / 2;
         for (int part = 0; part < 2; ++part) {
             split_groups.emplace_back(new Group());
@@ -1553,295 +1594,274 @@ static int eval_impl(bool dry, std::string *dump, bool json = false) {
             sub.phase = g.phase; sub.size = g.size;
             size_t lo = part == 0 ? 0 : half, hi = part == 0 ? half : g.roots.size();
             for (size_t r = lo; r < hi; ++r) plan.collect(sub, g.roots[r], nullptr);
-            if (!assemble_group(sub)) return false;
+            if (!assemble(sub)) return false;
         }
         return true;
-    };
-    for (auto &kv : plan.groups)                         /* ordered by (phase asc, size asc) */
-        if (!assemble_group(kv.second)) { ek_set_error("ek_eval(): " + asm_error); return -1; }
-    /* within a phase launch the largest size first (jit.cu:1450) */
-    std::stable_sort(launches.begin(), launches.end(), [](const auto &a, const auto &b) {
-        if (a.first->phase != b.first->phase) return a.first->phase < b.first->phase;
-        return a.first->size > b.first->size; });
+    }
+};
 
-    if (dry) {
-        std::ostringstream oss;
-        if (json) {
-            /* machine-readable form of the same listing for tests/ek_emulator.py (a numpy interpreter of the sweep ISA
-               that lets the CPU test-suite execute what the planner + assembler produce) */
-            oss << "{\"ops\":[";
-            for (int k = 0; k < DOP__COUNT; ++k) oss << (k ? "," : "") << "\"" << dop_name((uint16_t) k) << "\"";
-            oss << "],\"sweeps\":[";
-            bool first = true;
-            for (auto &l : launches) {
-                const Assembled &a = l.second;
-                oss << (first ? "" : ",") << "{\"phase\":" << l.first->phase << ",\"n\":" << l.first->size << ",\"n_tmp\":" << a.n_tmp;
-                first = false;
-                auto sec = [&](const char *name, const std::vector<EkInstr> &v) {
-                    oss << ",\"" << name << "\":[";
-                    for (size_t i = 0; i < v.size(); ++i)
-                        oss << (i ? "," : "") << "[" << v[i].op << "," << v[i].flags << "," << v[i].dst << "," << v[i].b << "," << v[i].c << "," << v[i].a << "," << v[i].imm << "]";
-                    oss << "]";
-                };
-                sec("init", a.init); sec("body", a.body); sec("fini", a.fini);
-                oss << ",\"lits\":[";
-                for (size_t i = 0; i < a.lits.size(); ++i) oss << (i ? "," : "") << a.lits[i];
-                oss << "],\"argw\":[";
-                for (size_t i = 0; i < a.argw.size(); ++i) oss << (i ? "," : "") << a.argw[i];
-                oss << "],\"ptr_fix\":[";
-                for (size_t i = 0; i < a.ptr_fix.size(); ++i) oss << (i ? "," : "") << "[" << a.ptr_fix[i].argw << "," << a.ptr_fix[i].var << "," << (a.ptr_fix[i].output ? 1 : 0) << "," << (unsigned long long) (uintptr_t) ctx.vars[a.ptr_fix[i].var].data << "]";
-                oss << "],\"staged\":[";
-                for (size_t i = 0; i < a.staged.size(); ++i) oss << (i ? "," : "") << "[" << a.staged[i].var << "," << a.staged[i].unit << "," << (int) a.staged[i].esize << "]";
-                oss << "],\"scalars\":[";
-                for (size_t i = 0; i < a.scalars.size(); ++i) oss << (i ? "," : "") << "[" << a.scalars[i].var << "," << (int) ctx.vars[a.scalars[i].var].type << "]";
-                oss << "],\"outputs\":[";
-                for (size_t i = 0; i < a.outputs.size(); ++i) oss << (i ? "," : "") << "[" << a.outputs[i].var << "," << a.outputs[i].argw << "," << a.outputs[i].bytes << "," << (int) ctx.vars[a.outputs[i].var].type << "]";
-                oss << "]";
-                {   /* the configuration the launcher picks for this sweep as it stands */
-                    Config lcfg; std::string lerr;
-                    if (choose_config(ctx, a, l.first->size, lcfg, lerr))
-                        oss << ",\"config\":{\"fast\":" << (lcfg.fast ? 1 : 0) << ",\"V\":" << lcfg.V << ",\"T\":" << lcfg.T
-                            << ",\"stages\":" << lcfg.stages << ",\"ctas_per_sm\":" << lcfg.ctas_per_sm << ",\"smem\":" << lcfg.smem
-                            << ",\"prog_in_smem\":" << (lcfg.prog_in_smem ? 1 : 0)
-                            << ",\"inline_prog\":" << (a.init.size() + a.body.size() + a.fini.size() <= EK_INLINE_PROG ? 1 : 0)
-                            << ",\"inline_lit\":" << (a.lits.size() <= EK_MAX_LIT_INLINE ? 1 : 0) << "}";
-                }
-                /* the program as the 32-bit fast kernel would receive it (lower_fast), when that is the kernel the
-                   launcher would pick for this sweep */
-                Config fcfg; std::string ferr;
-                /* (judged as a wide sweep whatever its size, so that small CPU test cases exercise the lowering too) */
-                if (choose_config(ctx, a, std::max<size_t>(l.first->size, 4097), fcfg, ferr) && fcfg.fast) {
-                    std::vector<EkInstr> fi, fb, ff;
-                    if (lower_fast(a.init, a, &fcfg, fi) && lower_fast(a.body, a, &fcfg, fb, a.release_at) && lower_fast(a.fini, a, &fcfg, ff)) {
-                        oss << ",\"fast\":{\"T\":" << fcfg.T << ",\"off_slots\":" << fcfg.off_slots << ",\"n_tmp\":" << a.n_tmp
-                            << ",\"off_bar\":" << fcfg.off_bar << ",\"off_extra\":" << fcfg.off_extra << ",\"smem\":" << fcfg.smem
-                            << ",\"n_in_units\":" << a.n_in_units << ",\"n_red\":" << a.n_red << ",\"argw\":[";
-                        {   /* argument words with the fast kernel's extra-region layout (pointer words still unpatched) */
-                            std::vector<uint32_t> aw(a.argw);
-                            layout_extra(a, fcfg, aw.data());
-                            for (size_t i = 0; i < aw.size(); ++i) oss << (i ? "," : "") << aw[i];
-                        }
-                        oss << "]";
-                        auto fsec = [&](const char *name, const std::vector<EkInstr> &v) {
-                            oss << ",\"" << name << "\":[";
-                            /* (fop, fflags, b, c, dst, aux, imm): see the field shuffle in lower_fast */
-                            for (size_t i = 0; i < v.size(); ++i)
-                                oss << (i ? "," : "") << "[" << v[i].op << "," << v[i].flags << "," << v[i].dst << "," << v[i].b << "," << v[i].c << "," << v[i].a << "," << v[i].imm << "]";
-                            oss << "]";
-                        };
-                        fsec("init", fi); fsec("body", fb); fsec("fini", ff);
-                        oss << ",\"release_mask\":" << (a.release_at >= 0 ? a.release_mask : 0u) << "}";
-                    }
-                }
-                oss << "}";
-            }
-            oss << "],\"configs\":{";
-            {   /* the candidate lists of choose_config, in the order it tries them */
-                auto cl = [&](const char *name, const Cand *c, size_t k, bool last) {
-                    oss << "\"" << name << "\":[";
-                    for (size_t i = 0; i < k; ++i) oss << (i ? "," : "") << "[" << c[i].V << "," << c[i].T << "," << c[i].stages << "," << c[i].want_ctas << "]";
-                    oss << "]" << (last ? "" : ",");
-                };
-                cl("small", small_cands, sizeof(small_cands) / sizeof(Cand), false);
-                cl("fast", fast_cands, sizeof(fast_cands) / sizeof(Cand), false);
-                cl("wide", wide_cands, sizeof(wide_cands) / sizeof(Cand), true);
-            }
-            oss << "},\"fops\":[";
-            {
-                static const char *fnames[] = { "NOP",
+/* machine-readable form of the ek_debug_plan() listing for tests/ek_emulator.py (a numpy interpreter of the sweep ISA
+   that lets the CPU test-suite execute what the planner + assembler produce) */
+void write_program_json(std::ostream &os, const EkContext &ctx, const std::vector<Sweep> &sweeps) {
+    auto instrs = [&](const char *name, const std::vector<EkInstr> &v) {
+        os << ",\"" << name << "\":[";
+        for (size_t i = 0; i < v.size(); ++i)
+            os << (i ? "," : "") << "[" << v[i].op << "," << v[i].flags << "," << v[i].dst << "," << v[i].b << "," << v[i].c << "," << v[i].a << "," << v[i].imm << "]";
+        os << "]";
+    };
+    os << "{\"ops\":[";
+    for (int k = 0; k < DOP__COUNT; ++k) os << (k ? "," : "") << "\"" << dop_name((uint16_t) k) << "\"";
+    os << "],\"sweeps\":[";
+    for (size_t si = 0; si < sweeps.size(); ++si) {
+        const Sweep &s = sweeps[si];
+        const Assembled &a = s.a;
+        os << (si ? "," : "") << "{\"phase\":" << s.g->phase << ",\"n\":" << s.g->size << ",\"n_tmp\":" << a.n_tmp;
+        instrs("init", a.init); instrs("body", a.body); instrs("fini", a.fini);
+        os << ",\"lits\":[";
+        for (size_t i = 0; i < a.lits.size(); ++i) os << (i ? "," : "") << a.lits[i];
+        os << "],\"argw\":[";
+        for (size_t i = 0; i < a.argw.size(); ++i) os << (i ? "," : "") << a.argw[i];
+        os << "],\"ptr_fix\":[";
+        for (size_t i = 0; i < a.ptr_fix.size(); ++i) os << (i ? "," : "") << "[" << a.ptr_fix[i].argw << "," << a.ptr_fix[i].var << "," << (a.ptr_fix[i].output ? 1 : 0) << "," << (unsigned long long) (uintptr_t) ctx.vars[a.ptr_fix[i].var].data << "]";
+        os << "],\"staged\":[";
+        for (size_t i = 0; i < a.staged.size(); ++i) os << (i ? "," : "") << "[" << a.staged[i].var << "," << a.staged[i].unit << "," << (int) a.staged[i].esize << "]";
+        os << "],\"scalars\":[";
+        for (size_t i = 0; i < a.scalars.size(); ++i) os << (i ? "," : "") << "[" << a.scalars[i].var << "," << (int) ctx.vars[a.scalars[i].var].type << "]";
+        os << "],\"outputs\":[";
+        for (size_t i = 0; i < a.outputs.size(); ++i) os << (i ? "," : "") << "[" << a.outputs[i].var << "," << a.outputs[i].argw << "," << a.outputs[i].bytes << "," << (int) ctx.vars[a.outputs[i].var].type << "]";
+        os << "]";
+        /* the configuration this sweep launches with, and the program it sends */
+        Program prog;
+        const bool expressible = kernel_program(a, s.cfg, prog);
+        os << ",\"config\":{\"fast\":" << (s.cfg.fast ? 1 : 0) << ",\"V\":" << s.cfg.V << ",\"T\":" << s.cfg.T
+           << ",\"stages\":" << s.cfg.stages << ",\"ctas_per_sm\":" << s.cfg.ctas_per_sm << ",\"smem\":" << s.cfg.smem
+           << ",\"prog_in_smem\":" << (s.cfg.prog_in_smem ? 1 : 0)
+           << ",\"inline_prog\":" << (prog.size() <= EK_INLINE_PROG ? 1 : 0)
+           << ",\"inline_lit\":" << (a.lits.size() <= EK_MAX_LIT_INLINE ? 1 : 0) << "}";
+        /* the program as the 32-bit fast kernel receives it: this sweep's own when it runs there; otherwise the one it
+           would receive if the sweep were wide (so that small CPU test cases exercise the lowering too), when the
+           launcher would then pick the fast kernel */
+        Config fcfg = s.cfg; Program fprog; std::string ferr;
+        const Program *fast = s.cfg.fast && expressible ? &prog : nullptr;
+        if (!s.cfg.fast && choose_config(ctx, a, std::max<size_t>(s.g->size, 4097), fcfg, ferr) && fcfg.fast && kernel_program(a, fcfg, fprog))
+            fast = &fprog;
+        if (fast) {
+            os << ",\"fast\":{\"T\":" << fcfg.T << ",\"off_slots\":" << fcfg.off_slots << ",\"n_tmp\":" << a.n_tmp
+               << ",\"off_bar\":" << fcfg.off_bar << ",\"off_extra\":" << fcfg.off_extra << ",\"smem\":" << fcfg.smem
+               << ",\"n_in_units\":" << a.n_in_units << ",\"n_red\":" << a.n_red << ",\"argw\":[";
+            std::vector<uint32_t> aw(a.argw.size());
+            argument_words(a, fcfg, aw.data());
+            for (size_t i = 0; i < aw.size(); ++i) os << (i ? "," : "") << aw[i];
+            os << "]";
+            /* (fop, fflags, b, c, dst, aux, imm): see the field shuffle in lower_fast */
+            instrs("init", fast->init); instrs("body", fast->body); instrs("fini", fast->fini);
+            os << ",\"release_mask\":" << (a.release_at >= 0 ? a.release_mask : 0u) << "}";
+        }
+        os << "}";
+    }
+    os << "],\"configs\":{";
+    {   /* the candidate lists of choose_config, in the order it tries them */
+        auto cl = [&](const char *name, const Cand *c, size_t k, bool last) {
+            os << "\"" << name << "\":[";
+            for (size_t i = 0; i < k; ++i) os << (i ? "," : "") << "[" << c[i].V << "," << c[i].T << "," << c[i].stages << "," << c[i].want_ctas << "]";
+            os << "]" << (last ? "" : ",");
+        };
+        cl("small", small_cands, sizeof(small_cands) / sizeof(Cand), false);
+        cl("fast", fast_cands, sizeof(fast_cands) / sizeof(Cand), false);
+        cl("wide", wide_cands, sizeof(wide_cands) / sizeof(Cand), true);
+    }
+    os << "},\"fops\":[";
+    {
+        static const char *fnames[] = { "NOP",
 #define X(n) #n, #n "_U",
-                    EK_FOPS2(X)
+            EK_FOPS2(X)
 #undef X
 #define X(n) #n,
-                    EK_FOPS1(X) EK_FOPS0(X)
+            EK_FOPS1(X) EK_FOPS0(X)
 #undef X
-                };
-                for (int k = 0; k < FOP__COUNT; ++k) oss << (k ? "," : "") << "\"" << fnames[k] << "\"";
-            }
-            oss << "]}";
-        } else {
-            for (auto &l : launches) dump_program(oss, l.second, *l.first);
-        }
-        if (dump) *dump = oss.str();
-        return 0;
+        };
+        for (int k = 0; k < FOP__COUNT; ++k) os << (k ? "," : "") << "\"" << fnames[k] << "\"";
     }
+    os << "]}";
+}
 
-    for (uint32_t idx : ctx.dirty) if (idx < ctx.vars.size()) ctx.vars[idx].dirty = false;   /* jit.cu:1430-1434 */
-    ctx.live.clear();
+/* ------------------------------------------------------------------ launch */
+/* the kernel arguments and grid of one sweep: allocates its outputs (jit.cu:1171-1174), passes the program and the
+   literals in the kernel parameters or through the program cache, and fills in the data pointers */
+bool sweep_args(EkContext &ctx, const Sweep &s, EkSweepArgs &args, uint32_t &grid, bool &inline_prog) {
+    const Assembled &a = s.a;
+    const Config &cfg = s.cfg;
+    for (const Output &o : a.outputs) {
+        EkVariable &v = ctx.vars[o.var];
+        if (v.data == nullptr) { v.data = ek_malloc(o.bytes); v.free_data = true; v.subtree_size = 1; }
+    }
+    Program prog;
+    if (!kernel_program(a, cfg, prog) || (cfg.fast && prog.size() > EK_INLINE_PROG)) {
+        ek_set_error("ek_eval(): internal error: fast-kernel lowering failed after it had been checked"); return false;
+    }
+    memset(&args, 0, sizeof(args));
+    inline_prog = prog.size() <= EK_INLINE_PROG;
+    const bool inline_lit = a.lits.size() <= EK_MAX_LIT_INLINE;
+    /* programs and literals that fit the kernel parameters travel there: nothing is uploaded and nothing is cached
+       (a trace whose literals change from step to step -- a step counter, a learning-rate schedule -- used to add a
+       cache entry and two synchronous uploads per step) */
+    if (!inline_prog || !inline_lit) lookup_program(ctx, prog, a.lits, !inline_prog, !inline_lit, args.prog, args.lit);
+    if (inline_prog) {
+        EkInstr *dstp = args.prog_inline;
+        for (const EkInstr &in : prog.init) *dstp++ = in;
+        for (const EkInstr &in : prog.body) *dstp++ = in;
+        for (const EkInstr &in : prog.fini) *dstp++ = in;
+    }
+    if (inline_lit && !a.lits.empty()) memcpy(args.lit_inline, a.lits.data(), a.lits.size() * 4);
+    if (inline_lit) args.lit = nullptr;
+    args.n_init = (uint32_t) prog.init.size(); args.n_body = (uint32_t) prog.body.size(); args.n_fini = (uint32_t) prog.fini.size();
+    args.n_lit = (uint32_t) a.lits.size();
+    args.n_argw = (uint32_t) a.argw.size();
+    args.n_scalar = (uint32_t) a.scalars.size();
+    args.n = (uint32_t) s.g->size;
+    uint32_t tile = cfg.T * cfg.V;
+    args.n_tiles = (uint32_t) ((s.g->size + tile - 1) / tile);
+    args.n_tmp = a.n_tmp; args.n_in_units = a.n_in_units;
+    args.n_staged = (uint32_t) a.staged.size();
+    args.n_stages = cfg.stages;
+    args.smem_bar_off = cfg.off_bar; args.smem_prog_off = cfg.off_prog;
+    args.smem_extra_off = cfg.off_extra; args.smem_slots_off = cfg.off_slots;
+    args.prog_in_smem = cfg.prog_in_smem ? 1 : 0;
+    args.n_red = a.n_red;
+    args.red_partials = ctx.red_partials; args.red_counters = ctx.red_counters;
+    args.tma_ok = 1;
+    for (size_t k = 0; k < a.staged.size(); ++k) {
+        const EkVariable &v = ctx.vars[a.staged[k].var];
+        if (v.data == nullptr) { ek_set_error("ek_eval(): internal error: staged input without data"); return false; }
+        args.staged_ptr[k] = v.data;
+        args.staged_unit[k] = a.staged[k].unit;
+        args.staged_esize[k] = a.staged[k].esize;
+        if (((uintptr_t) v.data & 15u) != 0) args.tma_ok = 0;
+    }
+    for (size_t k = 0; k < a.scalars.size(); ++k) {
+        const EkVariable &v = ctx.vars[a.scalars[k].var];
+        if (v.data == nullptr) { ek_set_error("ek_eval(): internal error: scalar input without data"); return false; }
+        args.scalar_ptr[k] = v.data;
+        args.scalar_type[k] = (uint8_t) v.type;
+    }
+    argument_words(a, cfg, args.argw);
+    for (const auto &pf : a.ptr_fix) {
+        uint64_t p = (uint64_t) (uintptr_t) ctx.vars[pf.var].data;
+        args.argw[pf.argw] = (uint32_t) p; args.argw[pf.argw + 1] = (uint32_t) (p >> 32);
+    }
+    grid = std::min<uint32_t>(args.n_tiles, (uint32_t) ctx.num_sms * cfg.ctas_per_sm);
+    grid = std::max(grid, 1u);
+    if (grid > ctx.max_grid) grid = ctx.max_grid;
+    return true;
+}
+
+bool launch_sweep(EkContext &ctx, const Sweep &s) {
+    const Assembled &a = s.a;
+    const Config &cfg = s.cfg;
+    EkSweepArgs args; uint32_t grid; bool inline_prog;
+    if (!sweep_args(ctx, s, args, grid, inline_prog)) return false;
+
+    if (ctx.log_level >= 1)
+        fprintf(stderr, "ek_eval(): launching sweep (n=%zu, in=%zu, out=%zu, ops=%u, slots=%u, V=%d, T=%u, stages=%u, grid=%u, smem=%zu)\n",
+                s.g->size, a.staged.size() + a.scalars.size(), a.outputs.size(), a.n_arith, a.n_tmp, cfg.V, cfg.T, cfg.stages, grid, cfg.smem);
+    if (ctx.log_level >= 3) { std::ostringstream oss; dump_program(oss, a, *s.g); fputs(oss.str().c_str(), stderr); }
+
+    if (ctx.timing) ek_cuda_check(cudaEventRecord(ctx.ev_start, ctx.stream));
+    if (cfg.fast) {
+        ek_cuda_check(ek_launch_sweep_fast(args, grid, cfg.T, cfg.smem, ctx.stream));
+    } else {
+        ek_cuda_check(ek_launch_sweep(cfg.V, inline_prog, args, grid, cfg.T, cfg.smem, ctx.stream));
+    }
+    if (ctx.timing) {
+        ek_cuda_check(cudaEventRecord(ctx.ev_stop, ctx.stream));
+        ek_cuda_check(cudaEventSynchronize(ctx.ev_stop));
+        float ms = 0; ek_cuda_check(cudaEventElapsedTime(&ms, ctx.ev_start, ctx.ev_stop));
+        ctx.stats.last_kernel_ms = ms; ctx.stats.total_kernel_ms += ms;
+    }
+    ctx.stats.launches++; ctx.stats.sweep_launches++;
+    if (cfg.fast) ctx.stats.fast_launches++;
+    ctx.stats.ops_evaluated += (uint64_t) a.n_arith * s.g->size;
+    ctx.stats.bytes_in += a.bytes_in; ctx.stats.bytes_out += a.bytes_out;
+    return true;
+}
+
+/* ------------------------------------------------------------------ releasing the trace */
+void clear_dirty(EkContext &ctx) {
+    for (uint32_t idx : ctx.dirty) if (idx < ctx.vars.size()) ctx.vars[idx].dirty = false;
     ctx.dirty.clear();
-    for (uint32_t idx : kept_literals) ctx.live.insert(idx);
+}
 
-    for (auto &l : launches) {
-        Group &g = *l.first;
-        Assembled &a = l.second;
-
-        Config cfg;
-        std::string err;
-        if (!choose_config(ctx, a, g.size, cfg, err)) { ek_set_error("ek_eval(): " + err); return -1; }
-
-        /* allocate outputs (jit.cu:1171-1174) */
-        for (const Output &o : a.outputs) {
-            EkVariable &v = ctx.vars[o.var];
-            if (v.data == nullptr) { v.data = ek_malloc(o.bytes); v.free_data = true; v.subtree_size = 1; }
-        }
-
-        /* operand codes -> (byte offset >> 4) for this configuration's shared-memory layout (general kernels; the fast
-           kernel's program is lowered from the symbolic form further down) */
-        const bool fast = cfg.fast;
-        if (!fast) {
-            const uint32_t slot_bytes = cfg.T * cfg.V * 4u;
-            auto patch = [&](uint16_t code) -> uint16_t {
-                if (code == EK_OPND_NONE || (code & EK_OPND_UNI)) return code;      /* uniform index == offset >> 4 */
-                if (code & EK_OPND_STAGED) return (uint16_t) (EK_OPND_STAGED | (((code & 0x3fffu) * slot_bytes) >> 4));
-                return (uint16_t) ((cfg.off_slots + (uint32_t) code * slot_bytes) >> 4);
-            };
-            auto patch_all = [&](std::vector<EkInstr> &v) {
-                for (EkInstr &in : v) {
-                    in.b = patch(in.b); in.c = patch(in.c);
-                    if (in.flags & EKF_HAS_A) in.a = patch(in.a);
-                    if ((in.flags & (EKF_ST | EKF_RACC)) || in.op == DOP_RACC) in.dst = patch(in.dst);
-                }
-            };
-            patch_all(a.init); patch_all(a.body); patch_all(a.fini);
-        }
-        EkSweepArgs args;
-        memset(&args, 0, sizeof(args));
-        std::vector<EkInstr> lowered_init, lowered_body, lowered_fini;
-        if (fast) {
-            if (!lower_fast(a.init, a, &cfg, lowered_init) || !lower_fast(a.body, a, &cfg, lowered_body, a.release_at) || !lower_fast(a.fini, a, &cfg, lowered_fini) ||
-                lowered_init.size() + lowered_body.size() + lowered_fini.size() > EK_INLINE_PROG) {
-                ek_set_error("ek_eval(): internal error: fast-kernel lowering failed after it had been checked"); return -1;
-            }
-        }
-        const std::vector<EkInstr> &p_init = fast ? lowered_init : a.init, &p_body = fast ? lowered_body : a.body, &p_fini = fast ? lowered_fini : a.fini;
-        const size_t n_prog_total = p_init.size() + p_body.size() + p_fini.size();
-        const bool inline_prog = n_prog_total <= EK_INLINE_PROG;
-        const bool inline_lit = a.lits.size() <= EK_MAX_LIT_INLINE;
-        /* programs and literals that fit the kernel parameters travel there: nothing is uploaded and nothing is cached
-           (a trace whose literals change from step to step -- a step counter, a learning-rate schedule -- used to add a
-           cache entry and two synchronous uploads per step) */
-        if (!inline_prog || !inline_lit) lookup_program(ctx, a, !inline_prog, !inline_lit, args.prog, args.lit);
-        if (inline_lit && !a.lits.empty()) memcpy(args.lit_inline, a.lits.data(), a.lits.size() * 4);
-        if (inline_lit) args.lit = nullptr;
-        args.n_init = (uint32_t) p_init.size(); args.n_body = (uint32_t) p_body.size(); args.n_fini = (uint32_t) p_fini.size();
-        args.n_lit = (uint32_t) a.lits.size();
-        args.n_argw = (uint32_t) a.argw.size();
-        args.n_scalar = (uint32_t) a.scalars.size();
-        args.n = (uint32_t) g.size;
-        uint32_t tile = cfg.T * cfg.V;
-        args.n_tiles = (uint32_t) ((g.size + tile - 1) / tile);
-        args.n_tmp = a.n_tmp; args.n_in_units = a.n_in_units;
-        args.n_staged = (uint32_t) a.staged.size();
-        args.n_stages = cfg.stages;
-        args.smem_bar_off = cfg.off_bar; args.smem_prog_off = cfg.off_prog;
-        args.smem_extra_off = cfg.off_extra; args.smem_slots_off = cfg.off_slots;
-        args.prog_in_smem = cfg.prog_in_smem ? 1 : 0;
-        args.n_red = a.n_red;
-        args.red_partials = ctx.red_partials; args.red_counters = ctx.red_counters;
-        args.tma_ok = 1;
-        for (size_t k = 0; k < a.staged.size(); ++k) {
-            const EkVariable &v = ctx.vars[a.staged[k].var];
-            if (v.data == nullptr) { ek_set_error("ek_eval(): internal error: staged input without data"); return -1; }
-            args.staged_ptr[k] = v.data;
-            args.staged_unit[k] = a.staged[k].unit;
-            args.staged_esize[k] = a.staged[k].esize;
-            if (((uintptr_t) v.data & 15u) != 0) args.tma_ok = 0;
-        }
-        for (size_t k = 0; k < a.scalars.size(); ++k) {
-            const EkVariable &v = ctx.vars[a.scalars[k].var];
-            if (v.data == nullptr) { ek_set_error("ek_eval(): internal error: scalar input without data"); return -1; }
-            args.scalar_ptr[k] = v.data;
-            args.scalar_type[k] = (uint8_t) v.type;
-        }
-        memcpy(args.argw, a.argw.data(), a.argw.size() * 4);
-        layout_extra(a, cfg, args.argw);             /* (fast kernel: offsets / copy counts of its own layout) */
-        for (const auto &pf : a.ptr_fix) {
-            uint64_t p = (uint64_t) (uintptr_t) ctx.vars[pf.var].data;
-            args.argw[pf.argw] = (uint32_t) p; args.argw[pf.argw + 1] = (uint32_t) (p >> 32);
-        }
-        uint32_t grid = std::min<uint32_t>(args.n_tiles, (uint32_t) ctx.num_sms * cfg.ctas_per_sm);
-        grid = std::max(grid, 1u);
-        if (grid > ctx.max_grid) grid = ctx.max_grid;
-
-        if (ctx.log_level >= 1)
-            fprintf(stderr, "ek_eval(): launching sweep (n=%zu, in=%zu, out=%zu, ops=%u, slots=%u, V=%d, T=%u, stages=%u, grid=%u, smem=%zu)\n",
-                    g.size, a.staged.size() + a.scalars.size(), a.outputs.size(), a.n_arith, a.n_tmp, cfg.V, cfg.T, cfg.stages, grid, cfg.smem);
-        if (ctx.log_level >= 3) { std::ostringstream oss; dump_program(oss, a, g); fputs(oss.str().c_str(), stderr); }
-
-        if (ctx.timing) ek_cuda_check(cudaEventRecord(ctx.ev_start, ctx.stream));
-        if (inline_prog) {
-            EkInstr *dstp = args.prog_inline;
-            for (const EkInstr &in : p_init) *dstp++ = in;
-            for (const EkInstr &in : p_body) *dstp++ = in;
-            for (const EkInstr &in : p_fini) *dstp++ = in;
-        }
-        if (fast) {
-            ek_cuda_check(ek_launch_sweep_fast(args, grid, cfg.T, cfg.smem, ctx.stream));
-        } else {
-            ek_cuda_check(ek_launch_sweep(cfg.V, inline_prog, args, grid, cfg.T, cfg.smem, ctx.stream));
-        }
-        if (ctx.timing) {
-            ek_cuda_check(cudaEventRecord(ctx.ev_stop, ctx.stream));
-            ek_cuda_check(cudaEventSynchronize(ctx.ev_stop));
-            float ms = 0; ek_cuda_check(cudaEventElapsedTime(&ms, ctx.ev_start, ctx.ev_stop));
-            ctx.stats.last_kernel_ms = ms; ctx.stats.total_kernel_ms += ms;
-        }
-        ctx.stats.launches++; ctx.stats.sweep_launches++;
-        if (fast) ctx.stats.fast_launches++;
-        ctx.stats.ops_evaluated += (uint64_t) a.n_arith * g.size;
-        ctx.stats.bytes_in += a.bytes_in; ctx.stats.bytes_out += a.bytes_out;
+/* clear the dependencies of `idx` and release the references they held */
+void drop_deps(EkContext &ctx, uint32_t idx) {
+    EkVariable &v = ctx.vars[idx];
+    uint32_t deps[4] = { v.dep[0], v.dep[1], v.dep[2], v.dep[3] };
+    uint32_t extra = v.extra_dep;
+    v.dep[0] = v.dep[1] = v.dep[2] = v.dep[3] = 0; v.extra_dep = 0;
+    for (int k = 0; k < 4; ++k) if (deps[k] >= EK_REG_RESERVED) {
+        /* dec_ref_int without re-entrancy surprises: var table may shrink but indices stay valid (the last reference
+           frees the variable through ek_dec_ref_ext) */
+        EkVariable &d = ctx.vars[deps[k]];
+        if (d.used && d.ref_int > 0) { if (--d.ref_int == 0 && d.ref_ext == 0) { d.ref_ext = 1; ek_dec_ref_ext(deps[k]); } }
     }
+    if (extra >= EK_REG_RESERVED) ek_dec_ref_ext(extra);
+}
 
-    /* post: drop dependencies of everything that now has data (jit.cu:1484-1507) */
-    std::vector<uint32_t> side_effects;
-    for (auto &l : launches) {
-        for (uint32_t idx : l.first->sched) {
+/* a side effect has run: drop its dependencies and release the reference the trace held */
+void retire_side_effect(EkContext &ctx, uint32_t idx) {
+    EkVariable &v = ctx.vars[idx];
+    v.side_effect = false;
+    v.op = EK_OP_INVALID;
+    drop_deps(ctx, idx);
+    ek_dec_ref_ext(idx);
+}
+
+/* after the launches: drop the dependencies of everything that now has data (jit.cu:1484-1507), then retire the side
+   effects that ran */
+void retire(EkContext &ctx, const Schedule &s) {
+    for (const Sweep &sw : s.sweeps) {
+        for (uint32_t idx : sw.g->sched) {
             if (idx >= ctx.vars.size() || !ctx.vars[idx].used) continue;
             EkVariable &v = ctx.vars[idx];
             if (v.data != nullptr && v.op != EK_OP_INVALID && !v.direct_pointer) {
-                uint32_t deps[4] = { v.dep[0], v.dep[1], v.dep[2], v.dep[3] };
-                uint32_t extra = v.extra_dep;
-                v.dep[0] = v.dep[1] = v.dep[2] = v.dep[3] = 0; v.extra_dep = 0;
                 v.op = EK_OP_INVALID;
-                for (int k = 0; k < 4; ++k) if (deps[k] >= EK_REG_RESERVED) {
-                    /* dec_ref_int without re-entrancy surprises: var table may shrink but indices stay valid */
-                    EkVariable &d = ctx.vars[deps[k]];
-                    if (d.used && d.ref_int > 0) { if (--d.ref_int == 0 && d.ref_ext == 0) { d.ref_ext = 1; ek_dec_ref_ext(deps[k]); } }
-                }
-                if (extra >= EK_REG_RESERVED) ek_dec_ref_ext(extra);
+                drop_deps(ctx, idx);
             }
         }
     }
-    for (auto &l : launches) {
-        for (uint32_t idx : l.first->sched) {
+    std::vector<uint32_t> side_effects;
+    for (const Sweep &sw : s.sweeps) {
+        for (uint32_t idx : sw.g->sched) {
             if (idx >= ctx.vars.size() || !ctx.vars[idx].used) continue;
             EkVariable &v = ctx.vars[idx];
             if (v.side_effect && v.op != EK_OP_INVALID) {
-                bool seen = std::find(side_effects.begin(), side_effects.end(), idx) != side_effects.end();
-                if (!seen) side_effects.push_back(idx);
+                if (std::find(side_effects.begin(), side_effects.end(), idx) == side_effects.end()) side_effects.push_back(idx);
             }
         }
     }
-    for (uint32_t idx : side_effects) {
-        EkVariable &v = ctx.vars[idx];
-        v.side_effect = false;          /* executed; release the reference the trace held */
-        v.op = EK_OP_INVALID;
-        uint32_t deps[4] = { v.dep[0], v.dep[1], v.dep[2], v.dep[3] };
-        uint32_t extra = v.extra_dep;
-        v.dep[0] = v.dep[1] = v.dep[2] = v.dep[3] = 0; v.extra_dep = 0;
-        for (int k = 0; k < 4; ++k) if (deps[k] >= EK_REG_RESERVED) {
-            EkVariable &d = ctx.vars[deps[k]];
-            if (d.used && d.ref_int > 0) { if (--d.ref_int == 0 && d.ref_ext == 0) { d.ref_ext = 1; ek_dec_ref_ext(deps[k]); } }
-        }
-        if (extra >= EK_REG_RESERVED) ek_dec_ref_ext(extra);
-        ek_dec_ref_ext(idx);
-    }
-    return 0;
+    for (uint32_t idx : side_effects) retire_side_effect(ctx, idx);
 }
 
+} // namespace
+
+/* ------------------------------------------------------------------ eval */
 extern "C" {
 
-int ek_eval(void) { return eval_impl(false, nullptr); }
+int ek_eval(void) {
+    EkContext &ctx = ek_ctx();
+    for (auto cb : ctx.callbacks) cb.first(cb.second);         /* jit.cu:1421-1422 */
+    if (ctx.live.empty()) { clear_dirty(ctx); return 0; }
+    if (ek_init() != 0) return -1;
+
+    Schedule s(ctx);
+    if (!s.build()) return -1;
+    clear_dirty(ctx);                                          /* jit.cu:1430-1434 */
+    ctx.live.clear();
+    for (uint32_t idx : s.kept_literals) ctx.live.insert(idx);
+    for (const Sweep &sw : s.sweeps)
+        if (!launch_sweep(ctx, sw)) return -1;
+    retire(ctx, s);
+    return 0;
+}
 
 int ek_eval_var(uint32_t index) {
     EkContext &ctx = ek_ctx();
@@ -1867,9 +1887,11 @@ int ek_eval_var(uint32_t index) {
 /* host-only: assemble what ek_eval() would launch and return a textual listing (malloc'd).
    Used by the CPU test-suite to check scheduling / register allocation without a GPU. */
 EK_API char *ek_debug_plan(void) {
-    std::string s;
-    if (eval_impl(true, &s) != 0) return nullptr;
-    return strdup(s.c_str());
+    Schedule s(ek_ctx());
+    if (!s.build()) return nullptr;
+    std::ostringstream oss;
+    for (const Sweep &sw : s.sweeps) dump_program(oss, sw.a, *sw.g);
+    return strdup(oss.str().c_str());
 }
 
 /* host-only test aid: forget recorded scatters that can never run (CPU test-suite without a GPU), exactly as if they
@@ -1879,29 +1901,18 @@ EK_API void ek_debug_discard_side_effects(void) {
     std::vector<uint32_t> pending;
     for (uint32_t idx : ctx.live)
         if (idx < ctx.vars.size() && ctx.vars[idx].used && ctx.vars[idx].side_effect && ctx.vars[idx].op != EK_OP_INVALID) pending.push_back(idx);
-    for (uint32_t idx : pending) {
-        EkVariable &v = ctx.vars[idx];
-        v.side_effect = false;
-        v.op = EK_OP_INVALID;
-        uint32_t deps[4] = { v.dep[0], v.dep[1], v.dep[2], v.dep[3] };
-        uint32_t extra = v.extra_dep;
-        v.dep[0] = v.dep[1] = v.dep[2] = v.dep[3] = 0; v.extra_dep = 0;
-        for (int k = 0; k < 4; ++k) if (deps[k] >= EK_REG_RESERVED) {
-            EkVariable &d = ctx.vars[deps[k]];
-            if (d.used && d.ref_int > 0) { if (--d.ref_int == 0 && d.ref_ext == 0) { d.ref_ext = 1; ek_dec_ref_ext(deps[k]); } }
-        }
-        if (extra >= EK_REG_RESERVED) ek_dec_ref_ext(extra);
-        ek_dec_ref_ext(idx);
-    }
-    for (uint32_t idx : ctx.dirty) if (idx < ctx.vars.size()) ctx.vars[idx].dirty = false;
-    ctx.dirty.clear();
+    for (uint32_t idx : pending) retire_side_effect(ctx, idx);
+    clear_dirty(ctx);
 }
 
-/* same as ek_debug_plan(), as JSON with the complete programs (tests/ek_emulator.py) */
+/* same as ek_debug_plan(), as JSON with the complete programs (tests/ek_emulator.py); empty when nothing is live */
 EK_API char *ek_debug_program(void) {
-    std::string s;
-    if (eval_impl(true, &s, true) != 0) return nullptr;
-    return strdup(s.c_str());
+    EkContext &ctx = ek_ctx();
+    Schedule s(ctx);
+    if (!s.build()) return nullptr;
+    std::ostringstream oss;
+    if (!ctx.live.empty()) write_program_json(oss, ctx, s.sweeps);
+    return strdup(oss.str().c_str());
 }
 
 } /* extern "C" */
