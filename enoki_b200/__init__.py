@@ -22,7 +22,7 @@ _OPS = ["INVALID", "LITERAL", "INDEX", "MOV", "CVT", "BITCAST", "NEG", "ABS", "S
         "EXP", "LOG", "SIN", "COS", "FLOOR", "CEIL", "ROUND", "TRUNC", "FLOOR2INT", "CEIL2INT", "NOT",
         "POPC", "CLZ", "CTZ", "ADD", "SUB", "MUL", "MULHI", "DIV", "MOD", "MIN", "MAX", "SHL", "SHR",
         "AND", "OR", "XOR", "GT", "GE", "LT", "LE", "EQ", "NE", "MUL_NZ", "FMA", "SELECT", "FMA_NZ",
-        "GATHER", "SCATTER", "SCATTER_ADD", "HSUM", "HPROD", "HMAX", "HMIN", "ALL", "ANY", "COUNT"]
+        "GATHER", "SCATTER", "SCATTER_ADD", "HSUM", "HPROD", "HMAX", "HMIN", "ALL", "ANY", "COUNT", "PRINTF"]
 OP = {n: i for i, n in enumerate(_OPS)}
 
 _NP = {EK_INT8: np.int8, EK_UINT8: np.uint8, EK_INT16: np.int16, EK_UINT16: np.uint16,
@@ -372,6 +372,18 @@ def partition(ptrs):
         libc.free.argtypes = [ctypes.c_void_p]
         libc.free(lists)
     return groups
+
+
+def cuda_printf(fmt, *args):
+    """enoki::cuda_printf (array_router.h:971-975): record a print of up to 3 arrays.  The evaluation that runs it
+    writes one line per element to C stdout, in recording order, with the values the arrays had when the print was
+    recorded.  The format is checked now (see ek_printf.cpp); a rejected one raises EnokiError and records nothing.
+    Print a DiffArray through detach(x)."""
+    for a in args:
+        if not isinstance(a, CUDAArray):
+            raise TypeError(f"cuda_printf(): arguments must be CUDA arrays, not {type(a).__name__}")
+    idx = (ctypes.c_uint32 * max(len(args), 1))(*[a.index for a in args])
+    _check(0, lib().ek_trace_printf(fmt.encode() if isinstance(fmt, str) else fmt, len(args), idx) == 0)
 
 
 def cuda_eval():

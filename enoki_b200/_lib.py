@@ -39,6 +39,7 @@ SIGNATURES = {
     "ek_set_device": (c_int, [c_int]),
     "ek_version": (ctypes.c_char_p, []),
     "ek_trace_append": (c_u32, [c_int, c_int, c_u32, c_u32, c_u32, c_u64]),
+    "ek_trace_printf": (c_int, [ctypes.c_char_p, c_u32, ctypes.POINTER(c_u32)]),
     "ek_inc_ref_ext": (None, [c_u32]),
     "ek_dec_ref_ext": (None, [c_u32]),
     "ek_var_size": (c_sz, [c_u32]),

@@ -1540,6 +1540,7 @@ struct Schedule {
     std::vector<std::unique_ptr<Group>> split_groups;
     std::vector<Sweep> sweeps;
     std::vector<uint32_t> kept_literals;      /* live literals: no sweep computes them, they stay live */
+    std::vector<uint32_t> prints;             /* print nodes (EK_OP_PRINTF), in recording order */
 
     explicit Schedule(EkContext &ctx) : plan(ctx) {}
 
@@ -1557,6 +1558,20 @@ struct Schedule {
             const EkVariable &v = ctx.vars[idx];
             if (!v.used) continue;
             if (v.data != nullptr && !v.side_effect) continue;
+            /* a print computes nothing itself: each computed argument becomes a root that its sweep must store (the
+               existing output store materialises it); evaluated and literal arguments are read as they are */
+            if (v.op == EK_OP_PRINTF) {
+                prints.push_back(idx);
+                for (int k = 0; k < 3; ++k) {
+                    uint32_t d = v.dep[k];
+                    if (d < EK_REG_RESERVED) continue;
+                    const EkVariable &dv = ctx.vars[d];
+                    if (dv.data != nullptr || dv.direct_pointer || dv.op == EK_OP_LITERAL) continue;
+                    plan.forced.insert(d);
+                    plan.add_root(d, work);
+                }
+                continue;
+            }
             /* literals are immediates: they are only given storage on demand (ek_eval_var) */
             if (v.op == EK_OP_LITERAL) { kept_literals.push_back(idx); continue; }
             plan.add_root(idx, work);
@@ -1600,9 +1615,22 @@ struct Schedule {
     }
 };
 
+/* `s` as a JSON string literal (the print formats of the dry runs) */
+void json_string(std::ostream &os, const std::string &s) {
+    os << '"';
+    for (unsigned char c : s) {
+        if (c == '"' || c == '\\') os << '\\' << c;
+        else if (c == '\n') os << "\\n";
+        else if (c == '\t') os << "\\t";
+        else if (c < 0x20) { char b[8]; snprintf(b, sizeof(b), "\\u%04x", c); os << b; }
+        else os << c;
+    }
+    os << '"';
+}
+
 /* machine-readable form of the ek_debug_plan() listing for tests/ek_emulator.py (a numpy interpreter of the sweep ISA
    that lets the CPU test-suite execute what the planner + assembler produce) */
-void write_program_json(std::ostream &os, const EkContext &ctx, const std::vector<Sweep> &sweeps) {
+void write_program_json(std::ostream &os, const EkContext &ctx, const std::vector<Sweep> &sweeps, const std::vector<uint32_t> &prints) {
     auto instrs = [&](const char *name, const std::vector<EkInstr> &v) {
         os << ",\"" << name << "\":[";
         for (size_t i = 0; i < v.size(); ++i)
@@ -1681,6 +1709,15 @@ void write_program_json(std::ostream &os, const EkContext &ctx, const std::vecto
 #undef X
         };
         for (int k = 0; k < FOP__COUNT; ++k) os << (k ? "," : "") << "\"" << fnames[k] << "\"";
+    }
+    os << "],\"prints\":[";
+    for (size_t i = 0; i < prints.size(); ++i) {
+        const EkVariable &v = ctx.vars[prints[i]];
+        os << (i ? "," : "") << "{\"fmt\":";
+        json_string(os, *v.fmt);
+        os << ",\"args\":[";
+        for (int k = 0, n = 0; k < 3; ++k) if (v.dep[k]) os << (n++ ? "," : "") << v.dep[k];
+        os << "],\"size\":" << v.size << "}";
     }
     os << "]}";
 }
@@ -1841,6 +1878,103 @@ void retire(EkContext &ctx, const Schedule &s) {
     for (uint32_t idx : side_effects) retire_side_effect(ctx, idx);
 }
 
+/* ------------------------------------------------------------------ prints (cuda_printf, jit.cu:863-916) */
+/* where one printed argument's values come from */
+struct PrintArg {
+    uint32_t var = 0;
+    ek_type type = EK_INVALID;
+    size_t size = 1;
+    bool immediate = false; uint64_t imm = 0;   /* literal / registered pointer: one value for every element */
+    void *snapshot = nullptr;                   /* evaluated before this eval: its copy, taken before the first launch */
+    std::vector<uint8_t> host;                  /* the values read back */
+};
+struct PrintJob { uint32_t node; std::vector<PrintArg> args; };
+
+/* Before the first launch.  Arguments that are already evaluated are copied in stream order, so that a scatter of the
+   same evaluation cannot change what is printed; computed arguments are stored by their sweeps (Planner::forced). */
+std::vector<PrintJob> snapshot_prints(EkContext &ctx, const std::vector<uint32_t> &prints) {
+    std::vector<PrintJob> jobs;
+    for (uint32_t idx : prints) {
+        PrintJob job; job.node = idx;
+        for (int k = 0; k < 3; ++k) {
+            uint32_t d = ctx.vars[idx].dep[k];
+            if (d < EK_REG_RESERVED) continue;
+            const EkVariable &dv = ctx.vars[d];
+            PrintArg a; a.var = d; a.type = dv.type; a.size = dv.size;
+            if (dv.direct_pointer) { a.immediate = true; a.imm = (uint64_t) (uintptr_t) dv.data; }
+            else if (dv.data == nullptr && dv.op == EK_OP_LITERAL) { a.immediate = true; a.imm = dv.imm; }
+            else if (dv.data != nullptr) {
+                size_t bytes = dv.size * ek_type_size(dv.type);
+                a.snapshot = ek_malloc(bytes);
+                ek_cuda_check(cudaMemcpyAsync(a.snapshot, dv.data, bytes, cudaMemcpyDeviceToDevice, ctx.stream));
+            }
+            job.args.push_back(std::move(a));
+        }
+        jobs.push_back(std::move(job));
+    }
+    return jobs;
+}
+
+/* After the launches: one synchronisation, the read-back of every argument, then the lines of each print in recording
+   order (elements ascending) on stdout, and one fflush. */
+void run_prints(EkContext &ctx, std::vector<PrintJob> &jobs) {
+    for (PrintJob &job : jobs)
+        for (PrintArg &a : job.args) {
+            if (a.immediate) continue;
+            const void *src = a.snapshot ? a.snapshot : ctx.vars[a.var].data;
+            if (!src) { fprintf(stderr, "ek_eval(): internal error: printed variable %u was not evaluated\n", a.var); exit(EXIT_FAILURE); }
+            a.host.resize(a.size * ek_type_size(a.type));
+            ek_cuda_check(cudaMemcpyAsync(a.host.data(), src, a.host.size(), cudaMemcpyDeviceToHost, ctx.stream));
+        }
+    ek_cuda_check(cudaStreamSynchronize(ctx.stream));
+    std::string out;
+    for (PrintJob &job : jobs) {
+        for (PrintArg &a : job.args) { ek_free(a.snapshot); a.snapshot = nullptr; }
+        const EkVariable &pv = ctx.vars[job.node];
+        const uint32_t narg = (uint32_t) job.args.size();
+        ek_type types[3] = { EK_INVALID, EK_INVALID, EK_INVALID };
+        for (uint32_t k = 0; k < narg; ++k) types[k] = job.args[k].type;
+        std::vector<EkPrintSeg> segs; std::string err;
+        if (!ek_printf_parse(pv.fmt->c_str(), narg, types, segs, err)) {     /* (checked when it was recorded) */
+            fprintf(stderr, "ek_eval(): internal error: %s\n", err.c_str()); exit(EXIT_FAILURE);
+        }
+        uint64_t bits[3] = { 0, 0, 0 };
+        for (size_t i = 0; i < pv.size; ++i) {
+            for (uint32_t k = 0; k < narg; ++k) {
+                const PrintArg &a = job.args[k];
+                if (a.immediate) { bits[k] = a.imm; continue; }
+                const size_t es = ek_type_size(a.type);
+                bits[k] = 0;
+                memcpy(&bits[k], a.host.data() + (a.size == 1 ? 0 : i) * es, es);
+            }
+            ek_printf_append(out, segs, types, bits);
+            if (out.size() >= ((size_t) 1 << 20)) { fwrite(out.data(), 1, out.size(), stdout); out.clear(); }
+        }
+    }
+    fwrite(out.data(), 1, out.size(), stdout);
+    fflush(stdout);
+}
+
+/* a print has run (or is discarded): free its format and release its arguments and the trace's reference */
+void retire_prints(EkContext &ctx, const std::vector<uint32_t> &prints) {
+    for (uint32_t idx : prints) {
+        delete ctx.vars[idx].fmt; ctx.vars[idx].fmt = nullptr;
+        retire_side_effect(ctx, idx);
+    }
+}
+
+/* the prints of the dry runs: format, argument handles and size */
+void dump_prints(std::ostream &os, const EkContext &ctx, const std::vector<uint32_t> &prints) {
+    for (uint32_t idx : prints) {
+        const EkVariable &v = ctx.vars[idx];
+        os << "print n=" << v.size << " args=";
+        for (int k = 0, n = 0; k < 3; ++k) if (v.dep[k]) os << (n++ ? "," : "") << v.dep[k];
+        os << " fmt=";
+        json_string(os, *v.fmt);
+        os << "\n";
+    }
+}
+
 } // namespace
 
 /* ------------------------------------------------------------------ eval */
@@ -1857,9 +1991,13 @@ int ek_eval(void) {
     clear_dirty(ctx);                                          /* jit.cu:1430-1434 */
     ctx.live.clear();
     for (uint32_t idx : s.kept_literals) ctx.live.insert(idx);
+    std::vector<PrintJob> jobs = snapshot_prints(ctx, s.prints);
     for (const Sweep &sw : s.sweeps)
         if (!launch_sweep(ctx, sw)) return -1;
+    /* (only an evaluation that prints waits for its launches) */
+    if (!jobs.empty()) run_prints(ctx, jobs);
     retire(ctx, s);
+    retire_prints(ctx, s.prints);
     return 0;
 }
 
@@ -1891,6 +2029,7 @@ EK_API char *ek_debug_plan(void) {
     if (!s.build()) return nullptr;
     std::ostringstream oss;
     for (const Sweep &sw : s.sweeps) dump_program(oss, sw.a, *sw.g);
+    dump_prints(oss, ek_ctx(), s.prints);
     return strdup(oss.str().c_str());
 }
 
@@ -1901,7 +2040,7 @@ EK_API void ek_debug_discard_side_effects(void) {
     std::vector<uint32_t> pending;
     for (uint32_t idx : ctx.live)
         if (idx < ctx.vars.size() && ctx.vars[idx].used && ctx.vars[idx].side_effect && ctx.vars[idx].op != EK_OP_INVALID) pending.push_back(idx);
-    for (uint32_t idx : pending) retire_side_effect(ctx, idx);
+    for (uint32_t idx : pending) { delete ctx.vars[idx].fmt; ctx.vars[idx].fmt = nullptr; retire_side_effect(ctx, idx); }
     clear_dirty(ctx);
 }
 
@@ -1911,7 +2050,7 @@ EK_API char *ek_debug_program(void) {
     Schedule s(ctx);
     if (!s.build()) return nullptr;
     std::ostringstream oss;
-    if (!ctx.live.empty()) write_program_json(oss, ctx, s.sweeps);
+    if (!ctx.live.empty()) write_program_json(oss, ctx, s.sweeps, s.prints);
     return strdup(oss.str().c_str());
 }
 

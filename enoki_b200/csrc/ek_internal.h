@@ -36,6 +36,7 @@ struct EkVariable {
     bool direct_pointer = false;
     bool used = false;                  /* slot in use */
     std::string *label = nullptr;
+    std::string *fmt = nullptr;         /* format of a print node (EK_OP_PRINTF), owned with it */
 };
 
 struct EkProgramCacheEntry {
@@ -128,3 +129,11 @@ static inline bool ek_is_signed(ek_type t) {
 static inline bool ek_is_64(ek_type t) { return ek_type_size(t) == 8; }
 const char *ek_type_name(ek_type t);
 const char *ek_op_name(ek_op op);
+
+/* cuda_printf formats (ek_printf.cpp).  A parsed format is a list of segments: literal text (conv == 0, "%%" already
+   reduced to "%") or one conversion, `text` being its spec as written ("%-08.3lx") and `arg` the argument it takes. */
+struct EkPrintSeg { std::string text; char conv; uint8_t len; /* 0 none, 1 hh, 2 h, 3 l, 4 ll */ uint8_t arg; };
+/* check `fmt` against the argument types; false (and `err`) when it is rejected */
+bool ek_printf_parse(const char *fmt, uint32_t narg, const ek_type *types, std::vector<EkPrintSeg> &segs, std::string &err);
+/* append one element's line: bits[k] = raw bits of argument k for that element (zero-extended) */
+void ek_printf_append(std::string &out, const std::vector<EkPrintSeg> &segs, const ek_type *types, const uint64_t *bits);

@@ -51,7 +51,7 @@ const char *ek_op_name(ek_op op) {
         "exp", "log", "sin", "cos", "floor", "ceil", "round", "trunc", "floor2int", "ceil2int", "not",
         "popc", "clz", "ctz", "add", "sub", "mul", "mulhi", "div", "mod", "min", "max", "shl", "shr",
         "and", "or", "xor", "gt", "ge", "lt", "le", "eq", "ne", "mul_nz", "fma", "select", "fma_nz",
-        "gather", "scatter", "scatter_add", "hsum", "hprod", "hmax", "hmin", "all", "any", "count" };
+        "gather", "scatter", "scatter_add", "hsum", "hprod", "hmax", "hmin", "all", "any", "count", "printf" };
     return (unsigned) op < EK_OP__COUNT ? names[op] : "?";
 }
 
@@ -115,7 +115,7 @@ void ek_shutdown(void) {
         cudaStreamSynchronize(ctx.stream);
         for (auto &v : ctx.vars) {
             if (v.used && v.data && v.free_data && !v.direct_pointer) cudaFree(v.data);
-            delete v.label;
+            delete v.label; delete v.fmt;
         }
         for (auto &kv : ctx.free_lists)
             for (void *p : kv.second) { if (kv.first.first == 2) cudaFreeHost(p); else cudaFree(p); }
@@ -358,7 +358,7 @@ static void var_free(uint32_t first) {
             if (dv.ref_ext == 0 && dv.ref_int == 0) work.push_back(v.extra_dep);
         }
         if (v.data && v.free_data && !v.direct_pointer) ek_free(v.data);
-        delete v.label;
+        delete v.label; delete v.fmt;
         v = EkVariable();
         ctx.free_handles.push_back(idx);
     }
@@ -555,6 +555,47 @@ uint32_t ek_trace_append(ek_type type, ek_op op, uint32_t a, uint32_t b, uint32_
         if (v.extra_dep >= EK_REG_RESERVED) ctx.vars[v.extra_dep].ref_ext++;
     }
     return idx;
+}
+
+/* jit.cu:863-916.  The node computes nothing: ek_eval() stores or snapshots its arguments and formats them on the host
+   (ek_printf.cpp) once the launches are done. */
+int ek_trace_printf(const char *fmt, uint32_t narg, const uint32_t *args) {
+    EkContext &ctx = ek_ctx();
+    if (narg > 3) { ek_set_error("cuda_trace_print(): at most 3 variables can be printed at once!"); return -1; }   /* jit.cu:912 */
+    ek_type types[3];
+    for (uint32_t k = 0; k < narg; ++k) {
+        if (args[k] == 0) { ek_set_error("ek_trace_printf(): arithmetic involving uninitialized variable!"); return -1; }   /* jit.cu:722-725 */
+        const EkVariable *v = var_get(args[k], "ek_trace_printf()");
+        if (!v) return -1;
+        if (v->side_effect) { ek_set_error("ek_trace_printf(): argument " + std::to_string(k + 1) + " is a side effect (scatter or print), not a value"); return -1; }
+        types[k] = v->type;
+    }
+    std::vector<EkPrintSeg> segs; std::string err;
+    if (!ek_printf_parse(fmt, narg, types, segs, err)) { ek_set_error(err); return -1; }
+    bool need_eval = false;
+    for (uint32_t k = 0; k < narg; ++k) if (ctx.vars[args[k]].dirty) need_eval = true;
+    if (need_eval && ek_eval() != 0) return -1;                                                     /* jit.cu:729-730 */
+    size_t size = 1;
+    for (uint32_t k = 0; k < narg; ++k) size = std::max(size, ctx.vars[args[k]].size);
+    for (uint32_t k = 0; k < narg; ++k) {
+        if (ctx.vars[args[k]].size != 1 && ctx.vars[args[k]].size != size) {                        /* jit.cu:776-782 */
+            std::string msg = "ek_trace_printf(): arithmetic involving arrays of incompatible size (";
+            for (uint32_t j = 0; j < narg; ++j) msg += (j ? (j + 1 == narg ? " and " : ", ") : "") + std::to_string(ctx.vars[args[j]].size);
+            ek_set_error(msg + "). The instruction was \"printf\".");
+            return -1;
+        }
+    }
+    uint32_t idx = var_new(EK_UINT32);
+    EkVariable &v = ctx.vars[idx];
+    v.op = EK_OP_PRINTF;
+    v.size = size;
+    v.subtree_size = 1;
+    for (uint32_t k = 0; k < narg; ++k) { v.dep[k] = args[k]; inc_ref_int(args[k]); }
+    v.fmt = new std::string(fmt);
+    v.side_effect = true;
+    v.ref_ext = 1;                      /* the trace's own reference, released when the print has run */
+    ctx.live.insert(idx);
+    return 0;
 }
 
 uint32_t ek_var_set_size(uint32_t index, size_t size, int copy) {

@@ -51,7 +51,8 @@ inline void cuda_shutdown() { ek_shutdown(); }
 /* (default arguments of cuda_eval / cuda_set_scatter_gather_operand come from the forward declarations in
    the reference's array_router.h:963-967) */
 inline void cuda_eval(bool /* log_assembly */) { detail::ek_chk_rc(ek_eval()); }
-inline void cuda_trace_printf(const char *, uint32_t, uint32_t *) { /* debugging aid of the PTX JIT (jit.cu:863-916): no-op */ }
+/* the reference's cuda_printf template (array_router.h:971-975) records through this; see ek_trace_printf() */
+inline void cuda_trace_printf(const char *fmt, uint32_t narg, uint32_t *args) { detail::ek_chk_rc(ek_trace_printf(fmt, narg, args)); }
 inline void cuda_eval_var(uint32_t index, bool = false) { detail::ek_chk_rc(ek_eval_var(index)); }
 inline void cuda_inc_ref_ext(uint32_t i) { ek_inc_ref_ext(i); }
 inline void cuda_dec_ref_ext(uint32_t i) { ek_dec_ref_ext(i); }
@@ -404,6 +405,8 @@ struct CUDAArray : ArrayBase<value_t<Value>, CUDAArray<Value>> {
     }
 
     Index index_() const { return m_index; }
+    /* the name the reference's cuda_printf template reads the handle by (array_router.h:973) */
+    Index index() const { return m_index; }
     size_t size() const { return m_index ? cuda_var_size(m_index) : 0; }
     bool empty() const { return size() == 0; }
     const Value *data() const { return (const Value *) cuda_var_ptr(m_index); }

@@ -114,6 +114,8 @@ typedef enum ek_op {
        and re-read the operand with CUB; semantics identical)                              */
     EK_OP_HSUM, EK_OP_HPROD, EK_OP_HMAX, EK_OP_HMIN,
     EK_OP_ALL, EK_OP_ANY, EK_OP_COUNT,
+    /* print node of ek_trace_printf() (jit.cu:863-916); not accepted by ek_trace_append()                  */
+    EK_OP_PRINTF,
     EK_OP__COUNT
 } ek_op;
 
@@ -131,6 +133,12 @@ EK_API const char *ek_version(void);
  * handle of SCATTER/SCATTER_ADD (4th operand).  Size/broadcast/dirty rules: jit.cu:701-861. */
 EK_API uint32_t ek_trace_append(ek_type type, ek_op op, uint32_t a, uint32_t b, uint32_t c,
                                 uint64_t imm);
+/* cuda.h:87-89 cuda_trace_printf (jit.cu:863-916): record a print of up to 3 arguments (any type but Float16).
+ * Sizes, broadcast and errors as ek_trace_append (no arguments: size 1).  The format is checked now (ek_printf.cpp
+ * lists what it may contain); a rejected format records nothing.  The evaluation that runs the print writes one
+ * line per element to stdout, in recording order, before it returns, with each argument's value at recording time.
+ * The library owns the node.  Returns 0, or -1 on a user error (ek_last_error()). */
+EK_API int      ek_trace_printf(const char *fmt, uint32_t narg, const uint32_t *args);
 EK_API void     ek_inc_ref_ext(uint32_t index);        /* cuda.h:41  (jit.cu:586-598) */
 EK_API void     ek_dec_ref_ext(uint32_t index);        /* cuda.h:44  (jit.cu:614-638) */
 EK_API size_t   ek_var_size(uint32_t index);           /* cuda.h:47 */
