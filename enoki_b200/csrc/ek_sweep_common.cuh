@@ -154,27 +154,30 @@ __device__ __forceinline__ int32_t f2i(float x, uint32_t mode) {
     }
 }
 __device__ __forceinline__ uint32_t f2u(float x, uint32_t mode) {
-    /* AVX2 has no unsigned conversion: the CPU path converts through int64/int32
-       (array_avx2.h); match cvttps2dq for the in-range case and wrap like a
-       64-bit truncation otherwise */
-    if (!(x > -9223372036854775808.f && x < 9223372036854775808.f)) return 0u;
-    long long v;
+    /* AVX2 has no unsigned conversion: the CPU path (array_avx2.h) converts a value r >= 2^31 as
+       cvttps2dq(r - 2^31) + 2^31 and anything else as cvttps2dq(r), where r = floor / ceil / trunc (x).  So r in
+       [0, 2^32) is exact, r in [-2^31, 0) wraps like int32, NaN and r < -2^31 give 0x80000000, r >= 2^32 gives 0 */
+    float r;
     switch (mode) {
-        case EK_RM: v = __float2ll_rd(x); break;
-        case EK_RP: v = __float2ll_ru(x); break;
-        case EK_RN: v = __float2ll_rn(x); break;
-        default:    v = __float2ll_rz(x); break;
+        case EK_RM: r = floorf(x); break;
+        case EK_RP: r = ceilf(x); break;
+        case EK_RN: r = rintf(x); break;
+        default:    r = truncf(x); break;
     }
-    return (uint32_t) v;
+    if (r >= 2147483648.f) return (uint32_t) f2i(r - 2147483648.f, EK_RZ) + 0x80000000u;
+    return (uint32_t) f2i(r, EK_RZ);
 }
+/* cvttpd2dq of the rounded value: the range test follows the rounding (ceil of a double just below 2^31 is out of range) */
 __device__ __forceinline__ int32_t d2i(double x, uint32_t mode) {
-    if (!(x >= -2147483648.0 && x < 2147483648.0)) return (int32_t) 0x80000000;
+    double r;
     switch (mode) {
-        case EK_RM: return __double2int_rd(x);
-        case EK_RP: return __double2int_ru(x);
-        case EK_RN: return __double2int_rn(x);
-        default:    return __double2int_rz(x);
+        case EK_RM: r = floor(x); break;
+        case EK_RP: r = ceil(x); break;
+        case EK_RN: r = rint(x); break;
+        default:    r = trunc(x); break;
     }
+    if (!(r >= -2147483648.0 && r < 2147483648.0)) return (int32_t) 0x80000000;
+    return __double2int_rz(r);
 }
 __device__ __forceinline__ long long d2ll(double x, uint32_t mode) {
     if (!(x >= -9223372036854775808.0 && x < 9223372036854775808.0)) return (long long) 0x8000000000000000ull;
@@ -193,6 +196,17 @@ __device__ __forceinline__ long long f2ll(float x, uint32_t mode) {
         case EK_RN: return __float2ll_rn(x);
         default:    return __float2ll_rz(x);
     }
+}
+/* to uint64: [2^63, 2^64) (where every float / double is an integer) is exact, anything else as the int64 conversion */
+__device__ __forceinline__ uint64_t f2ull(float x, uint32_t mode) {
+    if (x >= 9223372036854775808.f && x < 18446744073709551616.f)
+        return (uint64_t) f2ll(x - 9223372036854775808.f, EK_RZ) + 0x8000000000000000ull;
+    return (uint64_t) f2ll(x, mode);
+}
+__device__ __forceinline__ uint64_t d2ull(double x, uint32_t mode) {
+    if (x >= 9223372036854775808.0 && x < 18446744073709551616.0)
+        return (uint64_t) d2ll(x - 9223372036854775808.0, EK_RZ) + 0x8000000000000000ull;
+    return (uint64_t) d2ll(x, mode);
 }
 
 /* generic 64-bit-carried reduction combine (used by RACC slow path / RFIN) */

@@ -172,6 +172,55 @@ void ref_f2u(const float *in, uint32_t *out, size_t n) {
     memcpy(out, r.data(), n * 4);
 }
 
+/* ---- conversions between any two numeric types: DynamicArray<Packet<S, 8>> -> DynamicArray<Packet<D, 8>> through the
+        converting constructor (mode 0), floor2int<D> (1) or ceil2int<D> (2); type codes are the ek_type values ---- */
+} /* extern "C" */
+template <typename S, typename D> static int ref_convert_typed(int mode, const void *in, void *out, size_t n) {
+    using SX = DynamicArray<Packet<S, 8>>;
+    using DX = DynamicArray<Packet<D, 8>>;
+    SX x = SX::copy(in, n);
+    DX r;
+    if (mode == 0) r = DX(x);
+    else if constexpr (std::is_floating_point_v<S> && !std::is_floating_point_v<D>)
+        r = mode == 1 ? floor2int<DX>(x) : ceil2int<DX>(x);
+    else return -1;
+    memcpy(out, r.data(), n * sizeof(D));
+    return 0;
+}
+
+template <typename S> static int ref_convert_from(int dst, int mode, const void *in, void *out, size_t n) {
+    switch (dst) {
+        case 1:  return ref_convert_typed<S, int8_t>(mode, in, out, n);
+        case 2:  return ref_convert_typed<S, uint8_t>(mode, in, out, n);
+        case 3:  return ref_convert_typed<S, int16_t>(mode, in, out, n);
+        case 4:  return ref_convert_typed<S, uint16_t>(mode, in, out, n);
+        case 5:  return ref_convert_typed<S, int32_t>(mode, in, out, n);
+        case 6:  return ref_convert_typed<S, uint32_t>(mode, in, out, n);
+        case 7:  return ref_convert_typed<S, int64_t>(mode, in, out, n);
+        case 8:  return ref_convert_typed<S, uint64_t>(mode, in, out, n);
+        case 10: return ref_convert_typed<S, float>(mode, in, out, n);
+        case 11: return ref_convert_typed<S, double>(mode, in, out, n);
+        default: return -1;
+    }
+}
+extern "C" {
+
+int ref_convert(int src, int dst, int mode, const void *in, void *out, size_t n) {
+    switch (src) {
+        case 1:  return ref_convert_from<int8_t>(dst, mode, in, out, n);
+        case 2:  return ref_convert_from<uint8_t>(dst, mode, in, out, n);
+        case 3:  return ref_convert_from<int16_t>(dst, mode, in, out, n);
+        case 4:  return ref_convert_from<uint16_t>(dst, mode, in, out, n);
+        case 5:  return ref_convert_from<int32_t>(dst, mode, in, out, n);
+        case 6:  return ref_convert_from<uint32_t>(dst, mode, in, out, n);
+        case 7:  return ref_convert_from<int64_t>(dst, mode, in, out, n);
+        case 8:  return ref_convert_from<uint64_t>(dst, mode, in, out, n);
+        case 10: return ref_convert_from<float>(dst, mode, in, out, n);
+        case 11: return ref_convert_from<double>(dst, mode, in, out, n);
+        default: return -1;
+    }
+}
+
 /* ---- C1 (tests/dynamic.cpp path): r = a*b + sin(c), operator form ---- */
 void ref_c1(const float *a_, const float *b_, const float *c_, float *out, size_t n) {
     FloatX a = copy_f(a_, n), b = copy_f(b_, n), c = copy_f(c_, n);

@@ -81,6 +81,47 @@ def raise_fast(fast, fop_names, op_index):
     return {k: [conv(t) for t in fast[k]] for k in ("init", "body", "fini")}
 
 
+def _f2ll(x, mode, unsigned):
+    """float / double -> int64 (uint64) of the kernel: values outside [-2^63, 2^63) (for uint64 [-2^63, 2^64)) and NaN
+    give 0x8000000000000000, the rest is rounded in `mode` and wraps to 64 bits."""
+    r = {0: np.trunc, 1: np.floor, 2: np.ceil, 3: np.rint}[mode](x)
+    ok = (x >= -9.2233720368547758e18) & (x < 9.2233720368547758e18)
+    v = np.where(ok, np.where(ok, r, 0).astype(np.int64), np.int64(-9223372036854775808)).view(np.uint64)
+    if unsigned:
+        top = (x >= 9.2233720368547758e18) & (x < 1.8446744073709552e19)
+        v = np.where(top, (np.where(top, x, 0) - 9.2233720368547758e18).astype(np.int64).view(np.uint64) + np.uint64(1 << 63), v)
+    return v
+
+
+def _int64_ops(base, signed, ua, ub):
+    """64-bit mulhi, div / mod (ek_div64: /0 and INT64_MIN / -1 as the kernel guards them) and bit counts, in Python
+    integers."""
+    M = (1 << 64) - 1
+    sv = lambda v: v - (1 << 64) if signed and v >> 63 else v
+    out = []
+    for k in range(len(ua)):
+        a = int(ua[k]); b = int(ub[k]) if ub is not None else 0
+        if base in ("DIVR", "MODR"):
+            a, b = b, a
+        a, b = sv(a), sv(b)
+        if base == "MULHI": r = (a * b) >> 64
+        elif base == "POPC": r = bin(a & M).count("1")
+        elif base == "CLZ": r = 64 - (a & M).bit_length()
+        elif base == "CTZ": r = ((a & -a) & M).bit_length() - 1 if a & M else 64
+        elif base.startswith("DIV"):
+            if b == 0: r = 0 if signed else M
+            elif b == -1 and signed: r = -a
+            else:
+                q = abs(a) // abs(b); r = q if (a < 0) == (b < 0) else -q
+        else:
+            if b == 0: r = 0 if signed else a
+            elif b == -1 and signed: r = 0
+            else:
+                q = abs(a) // abs(b); r = a - (q if (a < 0) == (b < 0) else -q) * b
+        out.append(r & M)
+    return np.array(out, np.uint64)
+
+
 class Emulator:
     prefer_fast = False        # execute the lowered fast-kernel program of a sweep when the dump carries one
 
@@ -138,10 +179,12 @@ class Emulator:
             if name.endswith("_F64") and not name.startswith("CVT_"):
                 a = d(R, Rh); b = d(B, Bh) if Bh is not None else None; c = d(C, Ch) if Ch is not None else None
                 base = name[:-4]
-                if base in ("FMA", "FMAC"):
-                    x, y, z = (a, b, c) if base == "FMA" else (b, c, a)
+                if base in ("FMA", "FMAC", "FMANZ", "FMANZC"):
+                    x, y, z = (a, b, c) if base in ("FMA", "FMANZ") else (b, c, a)
                     x, y, z = (np.ascontiguousarray(v) for v in (x, y, z)); out = np.zeros_like(x)
                     self.oracle.or_fma_f64(_P(x), _P(y), _P(z), _P(out), SZ(len(x)))
+                    if base.startswith("FMANZ"):                      # a zero factor gives the addend as it is
+                        out = np.where((x == 0) | (y == 0), z, out)
                     return S(out)
                 if base in ("MIN", "MAX", "MINR", "MAXR"):
                     x, y = (a, b) if len(base) == 3 else (b, a)
@@ -154,6 +197,8 @@ class Emulator:
                 r = {"ADD": lambda: a + b, "SUB": lambda: a - b, "SUBR": lambda: b - a, "MUL": lambda: a * b, "DIV": lambda: a / b,
                      "DIVR": lambda: b / a, "ABS": lambda: np.abs(a), "NEG": lambda: -a, "SQRT": lambda: np.sqrt(a),
                      "FLOOR": lambda: np.floor(a), "CEIL": lambda: np.ceil(a), "ROUND": lambda: np.rint(a), "TRUNC": lambda: np.trunc(a),
+                     "RCP": lambda: 1.0 / a, "RSQRT": lambda: 1.0 / np.sqrt(a),
+                     "MULNZ": lambda: np.where((a == 0) | (b == 0), 0.0, a * b),
                      "EXP": lambda: self._unary64(2, a), "LOG": lambda: self._unary64(3, a), "SIN": lambda: self._unary64(0, a),
                      "COS": lambda: self._unary64(1, a)}.get(base)
                 if r is None:
@@ -184,6 +229,8 @@ class Emulator:
                 if base == "SEL_F": return np.where(B != 0, C, R), np.where(B != 0, Ch, Rh)
                 if base == "LOAD": return B, Bh
                 ua, ub = u(R, Rh), (u(B, Bh) if Bh is not None else None)
+                if base in ("MULHI", "DIV", "DIVR", "MOD", "MODR", "POPC", "CLZ", "CTZ"):
+                    return S(_int64_ops(base, signed, ua, ub))
                 r = {"ADD": lambda: ua + ub, "SUB": lambda: ua - ub, "SUBR": lambda: ub - ua, "MUL": lambda: ua * ub,
                      "MAD": lambda: ua * ub + u(C, Ch), "MADC": lambda: ub * u(C, Ch) + ua,
                      "MIN": lambda: np.minimum(a, b).view(np.uint64), "MAX": lambda: np.maximum(a, b).view(np.uint64),
@@ -206,21 +253,14 @@ class Emulator:
                 if name == "CVT_I64_F32": return i(R, Rh).astype(np.float32).view(np.uint32), Rh
                 if name == "CVT_U64_F32": return u(R, Rh).astype(np.float32).view(np.uint32), Rh
                 if name in ("CVT_F64_I64", "CVT_F64_U64", "CVT_F32_I64", "CVT_F32_U64"):
-                    if imm != 0:
-                        raise Unsupported("rounded conversion")
                     x = d(R, Rh) if "F64" in name else f32.astype(np.float64)
-                    ok = (x >= -9.2233720368547758e18) & (x < 9.2233720368547758e18)
-                    return S(np.where(ok, np.trunc(np.where(ok, x, 0)).astype(np.int64), np.int64(-9223372036854775808)).view(np.uint64))
-                if name in ("CVT_F64_I32",):
-                    x = d(R, Rh); ok = (x >= -2147483648.0) & (x < 2147483648.0)
-                    r = {0: np.trunc, 1: np.floor, 2: np.ceil, 3: np.rint}[imm](x)
+                    return S(_f2ll(x, imm, name.endswith("U64")))
+                if name in ("CVT_F64_I32",):                     # cvttpd2dq of the rounded value
+                    r = {0: np.trunc, 1: np.floor, 2: np.ceil, 3: np.rint}[imm](d(R, Rh))
+                    ok = (r >= -2147483648.0) & (r < 2147483648.0)
                     return np.where(ok, np.where(ok, r, 0).astype(np.int64), np.int64(-2147483648)).astype(np.int32).view(np.uint32), Rh
-                if name == "CVT_F64_U32":
-                    if imm != 0:
-                        raise Unsupported("rounded conversion")
-                    x = d(R, Rh); ok = (x >= -9.2233720368547758e18) & (x < 9.2233720368547758e18)
-                    v = np.where(ok, np.trunc(np.where(ok, x, 0)).astype(np.int64), np.int64(-9223372036854775808))
-                    return (v.view(np.uint64) & np.uint64(0xffffffff)).astype(np.uint32), Rh
+                if name == "CVT_F64_U32":                         # the low word of the int64 conversion
+                    return (_f2ll(d(R, Rh), imm, False) & np.uint64(0xffffffff)).astype(np.uint32), Rh
                 return None                                       # 32-bit conversions are handled by the caller
         return None
 
@@ -504,6 +544,10 @@ class Emulator:
                     var = var_of_uniform(imm)
                     self.vars[var] = (R & 0xff).astype(np.uint8).view(np.bool_) if out_type.get(var) == T_BOOL else (R & 0xff).astype(np.uint8)
                     return
+                elif name == "ST_16":
+                    var = var_of_uniform(imm)
+                    self.vars[var] = (R & 0xffff).astype(np.uint16)
+                    return
                 elif name == "NOT_32": R = ~R
                 elif name == "AND_32": R = R & B
                 elif name == "OR_32": R = R | B
@@ -529,11 +573,14 @@ class Emulator:
                 elif name == "LOAD_32": R = B
                 elif name == "INDEX": R = idx.copy()
                 elif name == "CVT_F32_U32":
-                    x = f(R)
-                    if imm != 0:
-                        raise Unsupported("rounded float->uint")
-                    ok = (x > -9.2233720368547758e18) & (x < 9.2233720368547758e18)
-                    R = np.where(ok, np.trunc(np.where(ok, x, 0)).astype(np.int64).astype(np.uint64) & np.uint64(0xffffffff), 0).astype(np.uint32)
+                    # the AVX2 sequence of the CPU path (array_avx2.h), after rounding:
+                    # r >= 2^31 ? cvttps2dq(r - 2^31) + 2^31 : cvttps2dq(r), cvttps2dq giving 0x80000000 out of range
+                    r = {0: np.trunc, 1: np.floor, 2: np.ceil, 3: np.rint}[imm](f(R)).astype(np.float64)
+                    hi = r >= 2147483648.0
+                    v = np.where(hi, r - 2147483648.0, r)
+                    ok = (v >= -2147483648.0) & (v < 2147483648.0)
+                    w = np.where(ok, np.where(ok, v, 0).astype(np.int64), np.int64(-2147483648)).astype(np.int32).view(np.uint32)
+                    R = np.where(hi, w + np.uint32(0x80000000), w)
                 elif name == "CVT_F32_I32":
                     x = f(R)
                     r = {0: np.trunc, 1: np.floor, 2: np.ceil, 3: np.rint}[imm](x)

@@ -96,8 +96,67 @@ def main():
     ref_math()
     ref_tape()
     ref_tape_sweep()
+    convert()
     shim_plan()
     print("golden vectors written to", HERE)
+
+
+# ek_type codes of the ten numeric types (include/enoki_b200.h)
+CONVERT_TYPES = {"Int8": 1, "UInt8": 2, "Int16": 3, "UInt16": 4, "Int32": 5, "UInt32": 6, "Int64": 7, "UInt64": 8,
+                 "Float32": 10, "Float64": 11}
+CONVERT_DTYPES = {"Int8": np.int8, "UInt8": np.uint8, "Int16": np.int16, "UInt16": np.uint16, "Int32": np.int32,
+                  "UInt32": np.uint32, "Int64": np.int64, "UInt64": np.uint64, "Float32": np.float32, "Float64": np.float64}
+
+
+def convert_inputs(rng, tname):
+    """One input vector per source type: the values where conversions change behaviour, then random ones."""
+    dt = np.dtype(CONVERT_DTYPES[tname])
+    if dt.kind == "f":
+        fi = np.finfo(dt)
+        v = [0.0, fi.smallest_subnormal, fi.smallest_normal - fi.smallest_subnormal, 0.5, 1.5, 2.5, 0.7, 1e19, 5e9, 3e9]
+        for e in (7, 8, 15, 16, 31, 32, 53, 63, 64):
+            b = dt.type(2.0 ** e)
+            v += [np.nextafter(b, dt.type(0)), b, np.nextafter(b, dt.type(np.inf))]
+        v = np.array(v, dt)
+        v = np.concatenate([v, -v, np.array([np.inf, -np.inf, np.nan], dt)])
+        emax = 128 if dt == np.float32 else 1024
+        emin = -149 if dt == np.float32 else -1074
+        mag = np.exp2(rng.uniform(emin, emax, 300)).astype(dt)
+        mag = np.where(np.isinf(mag), fi.max, mag)
+        sign = np.where(rng.random(300) < 0.5, -1, 1).astype(dt)
+        return np.concatenate([v, mag * sign, (rng.uniform(-300, 300, 100)).astype(dt)]).astype(dt)
+    info = np.iinfo(dt)
+    w = 8 * dt.itemsize
+    v = [info.min, info.max, -1, 0, 1, info.min + 1, info.max - 1]
+    for e in (24, 53):
+        v += [2 ** e - 1, 2 ** e + 1, -(2 ** e) - 1, -(2 ** e) + 1]
+    if w == 64:
+        v += [0x8000000000000001, 0x8000000000000000 + (1 << 40) + 1, 10 ** 19]
+    wrap = lambda x: np.array([int(x) & ((1 << w) - 1)], "u%d" % dt.itemsize).view(dt)[0]
+    v = np.array([wrap(x) for x in v if info.min <= x <= info.max or x >= 0 and info.min == 0 and x < 2 ** w], dt)
+    full = rng.integers(info.min, info.max, 200, endpoint=True, dtype=dt)
+    bits = rng.integers(1, w, 200)                       # magnitudes spread over every bit length
+    logu = np.array([wrap(int(rng.integers(0, 1 << 62)) % (1 << int(b)) * (-1 if info.min < 0 and k & 1 else 1))
+                     for k, b in enumerate(bits)], dt)
+    return np.concatenate([v, full, logu])
+
+
+def convert():
+    """The reference's conversions between every ordered pair of the ten numeric types (converting constructor), and
+    floor2int / ceil2int from Float32 and Float64 to the eight integer types (convert.npz).  x_<src> is the input of
+    source type src; <src>_<dst>_<mode> the output, mode 0 = converting constructor, 1 = floor2int, 2 = ceil2int."""
+    rng = np.random.default_rng(64)
+    d = {}
+    for src, sc in CONVERT_TYPES.items():
+        x = np.ascontiguousarray(convert_inputs(rng, src))
+        d[f"x_{src}"] = x
+        for dst, dc in CONVERT_TYPES.items():
+            modes = (0, 1, 2) if src.startswith("Float") and not dst.startswith("Float") else (0,)
+            for mode in modes:
+                out = np.zeros(len(x), CONVERT_DTYPES[dst])
+                assert R.ref_convert(sc, dc, mode, P(x), P(out), SZ(len(x))) == 0, (src, dst, mode)
+                d[f"{src}_{dst}_{mode}"] = out
+    np.savez_compressed(os.path.join(HERE, "convert.npz"), **d)
 
 
 # inputs of tests/test_cpu_oracle.py::test_oracle_vs_reference_math: (name, oracle selector, generator)
