@@ -27,7 +27,7 @@ OP = {n: i for i, n in enumerate(_OPS)}
 
 _NP = {EK_INT8: np.int8, EK_UINT8: np.uint8, EK_INT16: np.int16, EK_UINT16: np.uint16,
        EK_INT32: np.int32, EK_UINT32: np.uint32, EK_INT64: np.int64, EK_UINT64: np.uint64,
-       EK_FLOAT32: np.float32, EK_FLOAT64: np.float64, EK_BOOL: np.bool_}
+       EK_FLOAT16: np.float16, EK_FLOAT32: np.float32, EK_FLOAT64: np.float64, EK_BOOL: np.bool_}
 
 
 class EnokiError(RuntimeError):
@@ -70,7 +70,9 @@ class CUDAArray:
             h = lib().ek_var_copy_to_device(self.Type, arr.size, arr.ctypes.data)
             self.index = _check(h, h != 0)
         else:                                      # scalar literal, cuda.h:267-317
-            bits = np.array([value], dtype=_NP[self.Type]).view(
+            # (a Float16 literal is half(float(value)), the reference's converting constructor: two roundings)
+            val = np.array([value], dtype=np.float32 if self.Type == EK_FLOAT16 else _NP[self.Type]).astype(_NP[self.Type])
+            bits = val.view(
                 {1: np.uint8, 2: np.uint16, 4: np.uint32, 8: np.uint64}[np.dtype(_NP[self.Type]).itemsize])[0]
             self.index = _append(self.Type, "LITERAL", imm=int(bits))
 
@@ -213,6 +215,7 @@ def _make(name, t):
     return type(name, (CUDAArray,), {"Type": t, "__slots__": ()})
 
 
+Float16 = _make("Float16", EK_FLOAT16)     # storage only: convert to Float32 to compute (DESIGN.md 4)
 Float32 = _make("Float32", EK_FLOAT32)
 Float64 = _make("Float64", EK_FLOAT64)
 Int8 = _make("Int8", EK_INT8)
@@ -225,7 +228,7 @@ Int64 = _make("Int64", EK_INT64)
 UInt64 = _make("UInt64", EK_UINT64)
 Mask = _make("Mask", EK_BOOL)
 
-_BY_TYPE = {c.Type: c for c in (Float32, Float64, Int8, UInt8, Int16, UInt16, Int32, UInt32, Int64, UInt64, Mask)}
+_BY_TYPE = {c.Type: c for c in (Float16, Float32, Float64, Int8, UInt8, Int16, UInt16, Int32, UInt32, Int64, UInt64, Mask)}
 
 
 # ---- free functions (array_router.h / array_math.h names) -------------------------------

@@ -94,6 +94,7 @@ Cls cls_of(ek_type t) {
         case EK_FLOAT64: return C_F64;
         case EK_INT8: case EK_INT16: case EK_INT32: return C_I32;
         case EK_UINT8: case EK_UINT16: case EK_UINT32: case EK_BOOL: return C_U32;
+        case EK_FLOAT16: return C_U32;     /* its binary16 bits, moved like UInt16 (emit_var refuses arithmetic on them) */
         case EK_INT64: return C_I64;
         case EK_UINT64: case EK_POINTER: return C_U64;
         default: return C_BAD;
@@ -403,6 +404,20 @@ struct Assembler {
         return (uint32_t) lv.imm >= count;
     }
 
+    /* a staged Float16 input whose one use is a conversion to Float32 is not unpacked into a slot up front: the
+       conversion reads the staged tile itself (LD_U16 + CVT_F16_F32, one FOP_LD_F16 on the fast kernel) */
+    bool f16_read_by_cvt(uint32_t idx) const {
+        if (var(idx).type != EK_FLOAT16) return false;
+        int uses = 0; bool cvt = false;
+        for (uint32_t c : g.sched) {
+            const EkVariable &cv = var(c);
+            if (cv.data != nullptr || cv.direct_pointer || boundary_input(c) || cv.op == EK_OP_LITERAL || dead.count(c)) continue;
+            for (int k = 0; k < 4; ++k)
+                if (cv.dep[k] == idx) { ++uses; cvt = k == 0 && cv.op == EK_OP_CVT && cv.type == EK_FLOAT32; }
+        }
+        return uses == 1 && cvt;
+    }
+
     bool run() {
         /* ---- pass 0: masks implied by the range check of a shared-memory table / bins ---- */
         {
@@ -502,7 +517,7 @@ struct Assembler {
                     uint32_t units = es == 8 ? 2 : 1;
                     out.staged.push_back({ idx, (uint16_t) unit, (uint8_t) es });
                     loc[idx] = { Loc::STAGED, (uint16_t) unit };
-                    if (es != 4) unpack.push_back({ idx, i });
+                    if (es != 4 && !f16_read_by_cvt(idx)) unpack.push_back({ idx, i });
                     unit += units;
                     out.bytes_in += (uint64_t) v.size * es;
                 }
@@ -529,9 +544,8 @@ struct Assembler {
             switch (v.type) {
                 case EK_BOOL: case EK_UINT8: op = DOP_LD_U8; break;
                 case EK_INT8: op = DOP_LD_S8; break;
-                case EK_UINT16: op = DOP_LD_U16; break;
+                case EK_UINT16: case EK_FLOAT16: op = DOP_LD_U16; break;
                 case EK_INT16: op = DOP_LD_S16; break;
-                case EK_FLOAT16: return fail("Float16 arrays are not supported");
                 default: op = DOP_LD_64; break;
             }
             EkInstr in = mk(op);
@@ -555,9 +569,8 @@ struct Assembler {
                 switch (v.type) {
                     case EK_BOOL: case EK_UINT8: op = DOP_LDG_U8; break;
                     case EK_INT8: op = DOP_LDG_S8; break;
-                    case EK_UINT16: op = DOP_LDG_U16; break;
+                    case EK_UINT16: case EK_FLOAT16: op = DOP_LDG_U16; break;
                     case EK_INT16: op = DOP_LDG_S16; break;
-                    case EK_FLOAT16: return fail("Float16 arrays are not supported");
                     case EK_INT32: case EK_UINT32: case EK_FLOAT32: op = DOP_LDG_32; break;
                     default: op = DOP_LDG_64; break;
                 }
@@ -589,7 +602,15 @@ struct Assembler {
         uint32_t d0 = v.dep[0], d1 = v.dep[1], d2 = v.dep[2], d3 = v.dep[3];
 
         auto after = [&]() { if (d0) release(d0, pos); if (d1) release(d1, pos); if (d2) release(d2, pos); if (d3) release(d3, pos); };
-        if (t == EK_FLOAT16) return fail("Float16 arithmetic is not supported");
+        /* Float16 is a storage format (DESIGN.md §4): literals, conversions (incl. floor2int / ceil2int), bit casts,
+           select, gather and scatter move or convert its bits; everything else converts to Float32 first, as the
+           reference's half does */
+        if (op != EK_OP_LITERAL && op != EK_OP_MOV && op != EK_OP_CVT && op != EK_OP_FLOOR2INT && op != EK_OP_CEIL2INT &&
+            op != EK_OP_BITCAST && op != EK_OP_SELECT && op != EK_OP_GATHER && op != EK_OP_SCATTER) {
+            bool f16 = t == EK_FLOAT16;
+            for (int k = 0; k < 4; ++k) if (v.dep[k] >= EK_REG_RESERVED && var(v.dep[k]).type == EK_FLOAT16) f16 = true;
+            if (f16) return fail(std::string("op ") + ek_op_name(op) + " is not supported on Float16, a storage format: convert to Float32 to compute");
+        }
 
         /* ---------------- reductions ---------------- */
         if (is_reduce(op)) {
@@ -673,13 +694,31 @@ struct Assembler {
             case EK_OP_CVT: case EK_OP_FLOOR2INT: case EK_OP_CEIL2INT: {
                 ek_type st = var(d0).type;
                 int dop;
+                /* Float16 converts through Float32 (half(x) = float32_to_float16(float(x)), Value(h) = Value(float(h)) in the
+                   reference): `first` is the leg to or from Float32 that runs before `dop` */
+                int first = -1;
                 if (t == EK_BOOL && st != EK_BOOL) {
                     if (ek_is_float(st) || ek_is_64(st)) return fail("conversion to bool from this type is not supported");
                     dop = DOP_NEZ_32;
+                } else if (st == EK_FLOAT16 && t != EK_FLOAT16) {
+                    first = DOP_CVT_F16_F32;
+                    dop = pick_cvt(EK_FLOAT32, t);
+                } else if (t == EK_FLOAT16 && st != EK_FLOAT16) {
+                    first = st == EK_FLOAT32 ? -1 : pick_cvt(st, EK_FLOAT32);
+                    dop = DOP_CVT_F32_F16;
                 } else dop = pick_cvt(st, t);
                 if (dop < 0) return fail("unsupported conversion");
                 uint32_t mode = op == EK_OP_FLOOR2INT ? EK_RM : op == EK_OP_CEIL2INT ? EK_RP : EK_RZ;
-                ensure_acc(d0);
+                if (st == EK_FLOAT16 && loc[d0].kind == Loc::STAGED) {
+                    /* (f16_read_by_cvt: the staged tile is read here) */
+                    flush_pending();
+                    EkInstr ld = mk(DOP_LD_U16);
+                    ld.b = staged_code(loc[d0].idx);
+                    push_body(ld);
+                    acc_var = d0;
+                } else ensure_acc(d0);
+                if (first >= 0 && dop == DOP_LOAD_32) { dop = first; first = -1; }     /* Float16 -> Float32: one instruction */
+                if (first >= 0) push_body(mk(first));
                 in = mk(dop == DOP_LOAD_32 || dop == DOP_LOAD_64 ? DOP_NOP : dop, mode);
             } break;
             case EK_OP_BITCAST: {
@@ -698,7 +737,7 @@ struct Assembler {
                 switch (t) {
                     case EK_BOOL: case EK_UINT8: dop = DOP_GATHER_U8; break;
                     case EK_INT8: dop = DOP_GATHER_S8; break;
-                    case EK_UINT16: dop = DOP_GATHER_U16; break;
+                    case EK_UINT16: case EK_FLOAT16: dop = DOP_GATHER_U16; break;
                     case EK_INT16: dop = DOP_GATHER_S16; break;
                     case EK_INT32: case EK_UINT32: case EK_FLOAT32: dop = DOP_GATHER_32; break;
                     default: dop = DOP_GATHER_64; break;
@@ -871,6 +910,9 @@ struct Assembler {
         bool arith_narrow = (op >= EK_OP_NEG && op <= EK_OP_ABS) || (op >= EK_OP_ADD && op <= EK_OP_SHR) ||
                             op == EK_OP_FMA || op == EK_OP_NOT || op == EK_OP_CVT || op == EK_OP_FLOOR2INT || op == EK_OP_CEIL2INT;
         if (arith_narrow) nop = norm_op(t);
+        /* Float16 bits are held zero-extended, Int16 sign-extended: a bit cast between the two re-extends */
+        if (op == EK_OP_BITCAST && t == EK_FLOAT16 && var(d0).type == EK_INT16) nop = DOP_ZEXT16;
+        if (op == EK_OP_BITCAST && t == EK_INT16 && var(d0).type == EK_FLOAT16) nop = DOP_SEXT16;
 
         bool fused_mod = false;
         if (nop >= 0 && produces) {
@@ -1261,7 +1303,10 @@ bool lower_fast(const std::vector<EkInstr> &in, const Assembled &a, const Config
     };
     const size_t first = out.size();
     /* (emitted once every instruction lowered from in[release_at] is out: at the top of the next iteration) */
-    auto mark_release = [&](size_t j) { if (release_at >= 0 && j == (size_t) release_at + 1) emit(FOP_NOP, FF_REL, 0, 0, 0, 0, a.release_mask); };
+    bool released = false;
+    auto mark_release = [&](size_t j) {
+        if (!released && release_at >= 0 && j > (size_t) release_at) { emit(FOP_NOP, FF_REL, 0, 0, 0, 0, a.release_mask); released = true; }
+    };
     for (size_t j = 0; j < in.size(); ++j) {
         mark_release(j);
         const EkInstr &i = in[j];
@@ -1278,6 +1323,20 @@ bool lower_fast(const std::vector<EkInstr> &in, const Assembled &a, const Config
         if ((i.flags & EKF_NEG_A) && !fuse_neg) emit(FOP_NEG_F32, 0, 0, 0, 0, 0, 0);
         /* 2. the operation */
         int fop = fuse_neg ? FOP_EXPN_F32 : fuse_abs ? FOP_SQRTA_F32 : fop_of(i.op);
+        /* Float16 storage: a staged input read by its conversion (LD_U16; CVT_F16_F32) and an output stored by its
+           conversion (CVT_F32_F16; ST_16, when the next instruction reloads the accumulator or there is none: FOP_ST_F16
+           leaves the accumulator as it was) are one operation each; any other 16-bit instruction has no fast form.
+           `post` is the instruction whose post actions and imm the lowered operation carries. */
+        const EkInstr *post = &i;
+        if (j + 1 < in.size()) {
+            const EkInstr &nx = in[j + 1];
+            if (i.op == DOP_LD_U16 && i.flags == 0 && nx.op == DOP_CVT_F16_F32 &&
+                !(nx.flags & (EKF_HAS_A | EKF_NEG_A | EKF_ABS_A | EKF_HAS_B | EKF_HAS_C))) { fop = FOP_LD_F16; post = &nx; ++j; }
+            else if (i.op == DOP_CVT_F32_F16 && !(i.flags & (EKF_ST | EKF_STG | EKF_RACC)) && nx.op == DOP_ST_16 && nx.flags == 0 &&
+                     (j + 2 == in.size() || (in[j + 2].flags & EKF_HAS_A))) {
+                fop = FOP_ST_F16; post = &nx; ++j;
+            }
+        }
         if (fop < 0) return false;
         uint32_t fl = 0;
         uint16_t b = 0, c = 0, dst = 0, aux = 0;
@@ -1290,7 +1349,7 @@ bool lower_fast(const std::vector<EkInstr> &in, const Assembled &a, const Config
                 if (!hb) return false;
                 fop = ub ? FOP_LOADU : FOP_LOAD;
                 break;
-            case DOP_LD_U8: case DOP_LD_S8:                       /* raw staged code in b, no EKF_HAS_B */
+            case DOP_LD_U8: case DOP_LD_S8: case DOP_LD_U16:      /* raw staged code in b, no EKF_HAS_B (LD_U16: FOP_LD_F16) */
                 b = enc(i.b);
                 break;
             case DOP_GATHER_32: case DOP_GATHER_32_SMEM:          /* mask = B */
@@ -1331,16 +1390,17 @@ bool lower_fast(const std::vector<EkInstr> &in, const Assembled &a, const Config
                 break;
         }
         /* 3. post actions */
-        if (i.flags & EKF_ST) { fl |= FF_ST; dst = enc(i.dst); }
-        if (i.flags & EKF_STG) fl |= FF_STG;
-        if ((i.flags & EKF_RACC) || i.op == DOP_RACC) {
-            if (i.flags & EKF_ST) return false;
-            fl |= FF_RACC; dst = enc(i.dst);
-            aux = (uint16_t) (i.op == DOP_RACC ? (i.imm & 0xffffu) : i.a);
+        const EkInstr &p = *post;
+        if (p.flags & EKF_ST) { fl |= FF_ST; dst = enc(p.dst); }
+        if (p.flags & EKF_STG) fl |= FF_STG;
+        if ((p.flags & EKF_RACC) || p.op == DOP_RACC) {
+            if (p.flags & EKF_ST) return false;
+            fl |= FF_RACC; dst = enc(p.dst);
+            aux = (uint16_t) (p.op == DOP_RACC ? (p.imm & 0xffffu) : p.a);
             if (((aux >> 8) & 0xffu) > EK_RC_U32) return false;
         }
         if (i.op == DOP_NOP && !fl) continue;                    /* (a bare carrier of a load / modifier) */
-        emit((uint32_t) fop, fl, b, c, dst, aux, i.imm);
+        emit((uint32_t) fop, fl, b, c, dst, aux, p.imm);
     }
     mark_release(in.size());
     return true;
@@ -1705,7 +1765,7 @@ void write_program_json(std::ostream &os, const EkContext &ctx, const std::vecto
             EK_FOPS2(X)
 #undef X
 #define X(n) #n,
-            EK_FOPS1(X) EK_FOPS0(X)
+            EK_FOPS1(X) EK_FOPS0(X) EK_FOPS16(X)
 #undef X
         };
         for (int k = 0; k < FOP__COUNT; ++k) os << (k ? "," : "") << "\"" << fnames[k] << "\"";

@@ -114,6 +114,8 @@ struct EkInstr {
     X(CVT_F32_I64) X(CVT_F32_U64) X(CVT_F64_I64) X(CVT_F64_U64) \
     X(CVT_I64_F32) X(CVT_U64_F32) X(CVT_I64_F64) X(CVT_U64_F64) \
     X(CVT_I32_I64) X(CVT_U32_U64) X(CVT_64_32) \
+    /* Float16 storage: f32 -> binary16 bits (round to nearest even), binary16 bits -> f32 (exact) */ \
+    X(CVT_F32_F16) X(CVT_F16_F32) \
     /* staged-input unpack into the accumulator: b = staged operand code */ \
     X(LD_U8) X(LD_S8) X(LD_U16) X(LD_S16) X(LD_64) \
     /* direct (non-staged) loads into the accumulator: imm = uniform index of base pointer */ \
@@ -184,6 +186,10 @@ enum EkDop : uint16_t {
 #define EK_FOPS0(X) \
     X(SMEM_ZERO) X(SMEM_LOAD_TABLE) X(SMEM_FLUSH_ADD_F32) X(SMEM_FLUSH_ADD_I32) X(RFIN)
 
+/* Float16 storage, in the bodies that ek_fast16_kernel runs: LD_U16 + CVT_F16_F32 on a staged input, CVT_F32_F16 + ST_16
+   of an output (numbered last, so that the operations of ek_fast_kernel keep their numbers) */
+#define EK_FOPS16(X) X(LD_F16) X(ST_F16)
+
 enum EkFop : uint16_t {
     FOP_NOP,
 #define X(n) FOP_##n, FOP_##n##_U,
@@ -192,6 +198,7 @@ enum EkFop : uint16_t {
 #define X(n) FOP_##n,
     EK_FOPS1(X)
     EK_FOPS0(X)
+    EK_FOPS16(X)
 #undef X
     FOP__COUNT
 };

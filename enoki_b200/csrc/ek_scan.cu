@@ -162,6 +162,7 @@ void *ek_psum(ek_type type, size_t n, const void *data) {
         case EK_INT64: case EK_UINT64: return psum_impl<unsigned long long>(n, data);
         case EK_FLOAT32: return psum_impl<float>(n, data);
         case EK_FLOAT64: return psum_impl<double>(n, data);
+        case EK_FLOAT16: ek_set_error("ek_psum(): Float16 is a storage format: convert to Float32 to compute"); return nullptr;
         default: ek_set_error("ek_psum(): unsupported type"); return nullptr;
     }
 }

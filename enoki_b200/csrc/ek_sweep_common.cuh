@@ -6,6 +6,7 @@
 #pragma once
 #ifndef EK_HOST_EMU          /* tests/cpu_kernel: the fast kernel compiled as host code, see cuda_shim.h */
 #include <cuda_runtime.h>
+#include <cuda_fp16.h>
 #endif
 #include <stdint.h>
 #include "ek_isa.h"
@@ -208,6 +209,38 @@ __device__ __forceinline__ uint64_t d2ull(double x, uint32_t mode) {
         return (uint64_t) d2ll(x - 9223372036854775808.0, EK_RZ) + 0x8000000000000000ull;
     return (uint64_t) d2ll(x, mode);
 }
+
+/* Float16 is a storage format: a value is its binary16 bit pattern, zero-extended in a 32-bit register.  f32 -> f16
+   rounds to nearest even (cvt.rn.f16.f32: |x| >= 65520 gives inf, half subnormals exact, f32 subnormals give 0), the
+   reference's float32_to_float16 with F16C; f16 -> f32 is exact (cvt.f32.f16) */
+#ifdef EK_HOST_EMU
+/* (host build: the same two conversions in integer arithmetic, independent of the host's F16C; NaN gives the canonical
+   0x7fff / 0x7fffffff as on the H100) */
+inline uint32_t f32_to_f16(float f) {
+    uint32_t x; memcpy(&x, &f, 4);
+    const uint32_t sign = (x >> 16) & 0x8000u, ax = x & 0x7fffffffu;
+    if (ax > 0x7f800000u) return 0x7fffu;
+    if (ax >= 0x477ff000u) return sign | 0x7c00u;                                   /* |x| >= 65520: inf */
+    if (ax >= 0x38800000u) return sign | ((ax + 0xfffu + ((ax >> 13) & 1u) - 0x38000000u) >> 13);   /* normal half */
+    if (ax < 0x33000000u) return sign;                                              /* below 2^-25 (2^-25 ties to 0) */
+    const uint32_t shift = 126u - (ax >> 23), m = (ax & 0x7fffffu) | 0x800000u;     /* subnormal: m * 2^-shift units of 2^-24 */
+    uint32_t k = m >> shift;
+    const uint32_t rem = m & ((1u << shift) - 1u), halfway = 1u << (shift - 1u);
+    if (rem > halfway || (rem == halfway && (k & 1u))) ++k;
+    return sign | k;
+}
+inline float f16_to_f32(uint32_t h) {
+    const uint32_t sign = (h & 0x8000u) << 16, e = (h >> 10) & 0x1fu, m = h & 0x3ffu;
+    uint32_t x;
+    if (e == 0x1fu) x = m ? 0x7fffffffu : (sign | 0x7f800000u);
+    else if (e) x = sign | ((e + 112u) << 23) | (m << 13);
+    else { const float f = (float) m * 0x1p-24f; memcpy(&x, &f, 4); x |= sign; }
+    float r; memcpy(&r, &x, 4); return r;
+}
+#else
+__device__ __forceinline__ uint32_t f32_to_f16(float x) { return (uint32_t) __half_as_ushort(__float2half_rn(x)); }
+__device__ __forceinline__ float f16_to_f32(uint32_t h) { return __half2float(__ushort_as_half((unsigned short) h)); }
+#endif
 
 /* generic 64-bit-carried reduction combine (used by RACC slow path / RFIN) */
 __device__ __noinline__ uint64_t red_combine(uint32_t kind, uint32_t cls, uint64_t a, uint64_t b) {

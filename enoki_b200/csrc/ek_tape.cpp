@@ -99,6 +99,7 @@ void tape_eval_callback(void *p) {
 
 Tape *tape_of(ek_type t) {
     int i = t == EK_FLOAT64 ? 1 : 0;
+    if (t == EK_FLOAT16) { ek_set_error("tape: Float16 is a storage format: the value type must be Float32 or Float64"); return nullptr; }
     if (t != EK_FLOAT32 && t != EK_FLOAT64) { ek_set_error("tape: value type must be Float32 or Float64"); return nullptr; }
     if (!g_tapes[i]) {
         g_tapes[i] = new Tape(); g_tapes[i]->vt = t;

@@ -5,7 +5,7 @@ and the backend's stream is made explicit (synchronise the producer before the c
 import numpy as np
 
 from . import (CUDAArray, Float32, Float64, Int32, UInt32, Int64, UInt64, Mask, lib,
-               EK_FLOAT32, EK_FLOAT64, EK_INT32, EK_UINT32, EK_INT64, EK_UINT64, EK_BOOL)
+               EK_FLOAT16, EK_FLOAT32, EK_FLOAT64, EK_INT32, EK_UINT32, EK_INT64, EK_UINT64, EK_BOOL)
 
 
 def _torch():
@@ -15,7 +15,7 @@ def _torch():
 
 def _dtype_of(cls):
     t = _torch()
-    return {EK_FLOAT32: t.float32, EK_FLOAT64: t.float64, EK_INT32: t.int32, EK_UINT32: t.int32,
+    return {EK_FLOAT16: t.float16, EK_FLOAT32: t.float32, EK_FLOAT64: t.float64, EK_INT32: t.int32, EK_UINT32: t.int32,
             EK_INT64: t.int64, EK_UINT64: t.int64, EK_BOOL: t.bool}[cls.Type]
 
 

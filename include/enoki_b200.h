@@ -43,7 +43,8 @@ extern "C" {
 #  define EK_API __attribute__((visibility("default")))
 #endif
 
-/* Same numbering as enoki::EnokiType (include/enoki/array_traits.h:522-524) */
+/* Same numbering as enoki::EnokiType (include/enoki/array_traits.h:522-524).  EK_FLOAT16 (IEEE binary16) is a storage
+ * format: see ek_trace_append for what it accepts. */
 typedef enum ek_type {
     EK_INVALID = 0, EK_INT8, EK_UINT8, EK_INT16, EK_UINT16, EK_INT32, EK_UINT32,
     EK_INT64, EK_UINT64, EK_FLOAT16, EK_FLOAT32, EK_FLOAT64, EK_BOOL, EK_POINTER
@@ -130,7 +131,10 @@ EK_API const char *ek_version(void);
 /* ------------------------------------------------------------------ trace recording */
 /* cuda.h:65-89 cuda_trace_append (4 arities).  a/b/c = operand handles (0 = unused),
  * imm = literal bits (EK_OP_LITERAL), rounding/stride payload, or the `value` operand
- * handle of SCATTER/SCATTER_ADD (4th operand).  Size/broadcast/dirty rules: jit.cu:701-861. */
+ * handle of SCATTER/SCATTER_ADD (4th operand).  Size/broadcast/dirty rules: jit.cu:701-861.
+ * EK_FLOAT16 operands and results are accepted by LITERAL, MOV, CVT (through Float32, round to nearest even; not to Bool),
+ * FLOOR2INT / CEIL2INT, BITCAST (to / from 16-bit integers), SELECT, GATHER and SCATTER; any other operation on them
+ * is recorded but refused by the evaluation (ek_eval: an error naming Float16 -- convert to EK_FLOAT32 to compute). */
 EK_API uint32_t ek_trace_append(ek_type type, ek_op op, uint32_t a, uint32_t b, uint32_t c,
                                 uint64_t imm);
 /* cuda.h:87-89 cuda_trace_printf (jit.cu:863-916): record a print of up to 3 arguments (any type but Float16).
