@@ -22,7 +22,8 @@ _OPS = ["INVALID", "LITERAL", "INDEX", "MOV", "CVT", "BITCAST", "NEG", "ABS", "S
         "EXP", "LOG", "SIN", "COS", "FLOOR", "CEIL", "ROUND", "TRUNC", "FLOOR2INT", "CEIL2INT", "NOT",
         "POPC", "CLZ", "CTZ", "ADD", "SUB", "MUL", "MULHI", "DIV", "MOD", "MIN", "MAX", "SHL", "SHR",
         "AND", "OR", "XOR", "GT", "GE", "LT", "LE", "EQ", "NE", "MUL_NZ", "FMA", "SELECT", "FMA_NZ",
-        "GATHER", "SCATTER", "SCATTER_ADD", "HSUM", "HPROD", "HMAX", "HMIN", "ALL", "ANY", "COUNT", "PRINTF"]
+        "GATHER", "SCATTER", "SCATTER_ADD", "HSUM", "HPROD", "HMAX", "HMIN", "ALL", "ANY", "COUNT", "PRINTF",
+        "TAN", "COT", "ASIN", "ACOS", "ATAN", "ATAN2"]
 OP = {n: i for i, n in enumerate(_OPS)}
 
 _NP = {EK_INT8: np.int8, EK_UINT8: np.uint8, EK_INT16: np.int16, EK_UINT16: np.uint16,
@@ -243,6 +244,15 @@ sqrt, rcp, rsqrt, exp, log, sin, cos = (_unary(o) for o in ("SQRT", "RCP", "RSQR
 floor, ceil, round_, trunc = (_unary(o) for o in ("FLOOR", "CEIL", "ROUND", "TRUNC"))
 popcnt, lzcnt, tzcnt = (_unary(o) for o in ("POPC", "CLZ", "CTZ"))
 abs_ = _unary("ABS")
+# Float32 only: one node each, bit for bit the single precision branch of array_math.h (DESIGN.md 4)
+tan, cot, asin, acos, atan = (_unary(o) for o in ("TAN", "COT", "ASIN", "ACOS", "ATAN"))
+
+
+def atan2(y, x):
+    """atan2(y, x) (array_math.h:603-664); either operand may be a Python number"""
+    cls = next(type(v) for v in (y, x) if isinstance(v, CUDAArray))
+    y, x = (v if isinstance(v, CUDAArray) else cls(v) for v in (y, x))
+    return y._bin("ATAN2", x)
 
 
 def sincos(x):

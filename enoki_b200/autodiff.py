@@ -125,6 +125,7 @@ def _unary(label, f, dfdx):
 
 def _build():
     from . import sin as _sin, cos as _cos, exp as _exp, log as _log, sqrt as _sqrt, rcp as _rcp, Float32, UInt32, reinterpret
+    from . import tan as _tan, cot as _cot, asin as _asin, acos as _acos, atan as _atan, rsqrt as _rsqrt
 
     def _sign(a):
         # sign(a) = (sign_mask & a) | 1.0 (array_router.h:372): -1 at -0.0 and at NaNs with the sign bit set
@@ -138,6 +139,20 @@ def _build():
     g["sqrt"] = _unary("sqrt", _sqrt, lambda a, r: Float32(0.5) / r)       # autodiff.h:353-364
     g["rcp"] = _unary("rcp", _rcp, lambda a, r: -(r * r))                  # autodiff.h:379-390
     g["abs"] = _unary("abs", lambda a: abs(a), lambda a, r: _sign(a))      # autodiff.h:341-351
+
+    def _sqr_sec(a):
+        s = _rcp(_cos(a))
+        return s * s
+
+    def _neg_sqr_csc(a):
+        c = _rcp(_sin(a))
+        return -(c * c)
+
+    g["tan"] = _unary("tan", _tan, lambda a, r: _sqr_sec(a))                    # autodiff.h:532-542: sqr(sec(a))
+    g["cot"] = _unary("cot", _cot, lambda a, r: _neg_sqr_csc(a))                # autodiff.h:570-580: -sqr(csc(a))
+    g["asin"] = _unary("asin", _asin, lambda a, r: _rsqrt(1.0 - a * a))         # autodiff.h:582-592
+    g["acos"] = _unary("acos", _acos, lambda a, r: -_rsqrt(1.0 - a * a))        # autodiff.h:594-604
+    g["atan"] = _unary("atan", _atan, lambda a, r: _rcp(1.0 + a * a))           # autodiff.h:606-616
     return g
 
 
@@ -158,6 +173,22 @@ def log(x): return _op("log")(x)
 def sqrt(x): return _op("sqrt")(x)
 def rcp(x): return _op("rcp")(x)
 def abs_(x): return _op("abs")(x)
+def tan(x): return _op("tan")(x)
+def cot(x): return _op("cot")(x)
+def asin(x): return _op("asin")(x)
+def acos(x): return _op("acos")(x)
+def atan(x): return _op("atan")(x)
+
+
+def atan2(y, x):
+    """autodiff.h:618-633: il2 = rcp(sqr(y) + sqr(x)), weights (il2 * x, -il2 * y)."""
+    from . import atan2 as _atan2, rcp as _rcp
+    y, x = FloatD._c(y), FloatD._c(x)
+    r = _atan2(y.value, x.value)
+    if y.index == 0 and x.index == 0:
+        return FloatD(r, 0)
+    il2 = _rcp(y.value * y.value + x.value * x.value)
+    return FloatD._node("atan2", r, [y, x], [il2 * x.value, -il2 * y.value])
 
 
 def fmadd(a, b, c):

@@ -130,6 +130,12 @@ int pick_op(ek_op op, ek_type vt, ek_type at /* operand type */) {
         case EK_OP_LOG:   return SEL(DOP_LOG_F32, DOP_LOG_F64, -1, -1, -1, -1);
         case EK_OP_SIN:   return SEL(DOP_SIN_F32, DOP_SIN_F64, -1, -1, -1, -1);
         case EK_OP_COS:   return SEL(DOP_COS_F32, DOP_COS_F64, -1, -1, -1, -1);
+        case EK_OP_TAN:   return SEL(DOP_TAN_F32, -1, -1, -1, -1, -1);
+        case EK_OP_COT:   return SEL(DOP_COT_F32, -1, -1, -1, -1, -1);
+        case EK_OP_ASIN:  return SEL(DOP_ASIN_F32, -1, -1, -1, -1, -1);
+        case EK_OP_ACOS:  return SEL(DOP_ACOS_F32, -1, -1, -1, -1, -1);
+        case EK_OP_ATAN:  return SEL(DOP_ATAN_F32, -1, -1, -1, -1, -1);
+        case EK_OP_ATAN2: return SEL(DOP_ATAN2_F32, -1, -1, -1, -1, -1);
         case EK_OP_FLOOR: return SEL(DOP_FLOOR_F32, DOP_FLOOR_F64, DOP_LOAD_32, DOP_LOAD_32, DOP_LOAD_64, DOP_LOAD_64);
         case EK_OP_CEIL:  return SEL(DOP_CEIL_F32, DOP_CEIL_F64, DOP_LOAD_32, DOP_LOAD_32, DOP_LOAD_64, DOP_LOAD_64);
         case EK_OP_ROUND: return SEL(DOP_ROUND_F32, DOP_ROUND_F64, DOP_LOAD_32, DOP_LOAD_32, DOP_LOAD_64, DOP_LOAD_64);
@@ -205,8 +211,8 @@ uint64_t red_identity(int kind, int cls) {
 uint32_t acc_positions(const EkVariable &v) {
     ek_op op = v.op;
     if (op == EK_OP_LITERAL || op == EK_OP_INDEX) return 0;
-    if (op >= EK_OP_MOV && op <= EK_OP_CTZ) return 1;
-    if (op >= EK_OP_ADD && op <= EK_OP_MUL_NZ) return 3;
+    if (ek_op_unary(op)) return 1;
+    if (ek_op_binary(op)) return 3;
     if (op == EK_OP_FMA || op == EK_OP_SELECT || op == EK_OP_FMA_NZ) return 7;
     if (op == EK_OP_GATHER || op == EK_OP_SCATTER || op == EK_OP_SCATTER_ADD) return 2;   /* the index */
     if (op >= EK_OP_HSUM && op <= EK_OP_COUNT) return 1;
@@ -872,13 +878,13 @@ struct Assembler {
                 }
             }   /* fall through */
             default: {
-                if (op >= EK_OP_MOV && op <= EK_OP_CTZ) {                 /* unary */
+                if (ek_op_unary(op)) {                                    /* unary */
                     ek_type at = var(d0).type;
                     int dop = pick_op(op, t, at);
                     if (dop < 0) return fail(std::string("op ") + ek_op_name(op) + " not supported for type " + ek_type_name(t));
                     ensure_acc(d0);
                     in = mk(dop == DOP_LOAD_32 || dop == DOP_LOAD_64 ? DOP_NOP : dop);
-                } else if (op >= EK_OP_ADD && op <= EK_OP_MUL_NZ) {       /* binary */
+                } else if (ek_op_binary(op)) {                            /* binary */
                     ek_type at = var(d0).type;
                     int p = acc_at(d0, d1, 0);
                     if (p < 0) { ensure_acc(d0); p = 0; }
@@ -890,7 +896,7 @@ struct Assembler {
                             case EK_OP_GE: eop = EK_OP_LE; break;
                             case EK_OP_LT: eop = EK_OP_GT; break;
                             case EK_OP_LE: eop = EK_OP_GE; break;
-                            case EK_OP_SUB: case EK_OP_DIV: case EK_OP_MOD: case EK_OP_SHL: case EK_OP_SHR: reversed = true; break;
+                            case EK_OP_SUB: case EK_OP_DIV: case EK_OP_MOD: case EK_OP_SHL: case EK_OP_SHR: case EK_OP_ATAN2: reversed = true; break;
                             case EK_OP_MIN: case EK_OP_MAX: reversed = ek_is_float(t); break;
                             default: break;       /* commutative */
                         }
@@ -984,6 +990,7 @@ struct Assembler {
 
     /* does the instruction leave its imm field unused (so that EKF_STG can use it)? */
     static bool imm_free(int op) {
+        if (op >= DOP_TAN_F32 && op <= DOP_ATAN2R_F32) return true;
         if (op >= DOP_CVT_F32_I32 && op <= DOP_CVT_64_32) return false;
         if (op >= DOP_LD_U8) return false;          /* loads, stores, gathers, scatters, reductions, smem helpers */
         return true;
@@ -1007,7 +1014,7 @@ struct Assembler {
 
     static int reversed_op(int dop) {
         switch (dop) {
-            case DOP_SUB_F32: return DOP_SUBR_F32; case DOP_DIV_F32: return DOP_DIVR_F32;
+            case DOP_SUB_F32: return DOP_SUBR_F32; case DOP_DIV_F32: return DOP_DIVR_F32; case DOP_ATAN2_F32: return DOP_ATAN2R_F32;
             case DOP_MIN_F32: return DOP_MINR_F32; case DOP_MAX_F32: return DOP_MAXR_F32;
             case DOP_SUB_F64: return DOP_SUBR_F64; case DOP_DIV_F64: return DOP_DIVR_F64;
             case DOP_MIN_F64: return DOP_MINR_F64; case DOP_MAX_F64: return DOP_MAXR_F64;
@@ -1048,6 +1055,8 @@ struct Assembler {
         /* heavier instructions weigh more: transcendental ~ 8, others 1 */
         auto weight = [&](const EkInstr &in) -> double {
             switch (in.op) { case DOP_SIN_F32: case DOP_COS_F32: case DOP_EXP_F32: case DOP_LOG_F32: return 8.0;
+                             case DOP_TAN_F32: case DOP_COT_F32: return 12.0;
+                             case DOP_ASIN_F32: case DOP_ACOS_F32: case DOP_ATAN_F32: case DOP_ATAN2_F32: case DOP_ATAN2R_F32: return 10.0;
                              case DOP_SQRT_F32: case DOP_DIV_F32: case DOP_RCP_F32: case DOP_RSQRT_F32: return 3.0; default: return 1.0; } };
         double total_w = 0; for (const EkInstr &in : out.body) total_w += weight(in);
         double acc_w = 0;
@@ -1264,6 +1273,7 @@ int fop_of(int dop) {
         X(GATHER_32) X(GATHER_32_SMEM) X(SCATTER_32) X(SCATTER_ADD_F32) X(SCATTER_ADD_I32)
         X(SCATTER_ADD_F32_SMEM) X(SCATTER_ADD_I32_SMEM) X(RACC)
         EK_FOPS0(X)
+        X(TAN_F32) X(COT_F32) X(ASIN_F32) X(ACOS_F32) X(ATAN_F32) X(ATAN2_F32) X(ATAN2R_F32)
 #undef X
         case DOP_LOAD_32: return FOP_LOAD;
         default: return -1;
@@ -1274,6 +1284,7 @@ bool fop_has_u_twin(int fop) {
 #define X(n) case FOP_##n:
         EK_FOPS2(X)
 #undef X
+        case FOP_ATAN2_F32: case FOP_ATAN2R_F32:
             return true;
         default: return false;
     }
@@ -1743,7 +1754,9 @@ void write_program_json(std::ostream &os, const EkContext &ctx, const std::vecto
             os << "]";
             /* (fop, fflags, b, c, dst, aux, imm): see the field shuffle in lower_fast */
             instrs("init", fast->init); instrs("body", fast->body); instrs("fini", fast->fini);
-            os << ",\"release_mask\":" << (a.release_at >= 0 ? a.release_mask : 0u) << "}";
+            /* ext: the EK_FX_* operation sets of the body, i.e. the instantiation ek_fast_kernel<T, ext> that runs it */
+            os << ",\"release_mask\":" << (a.release_at >= 0 ? a.release_mask : 0u)
+               << ",\"ext\":" << ek_fast_ext(fast->body.data(), (uint32_t) fast->body.size()) << "}";
         }
         os << "}";
     }
@@ -1765,7 +1778,7 @@ void write_program_json(std::ostream &os, const EkContext &ctx, const std::vecto
             EK_FOPS2(X)
 #undef X
 #define X(n) #n,
-            EK_FOPS1(X) EK_FOPS0(X) EK_FOPS16(X)
+            EK_FOPS1(X) EK_FOPS0(X) EK_FOPS16(X) EK_FOPST(X)
 #undef X
         };
         for (int k = 0; k < FOP__COUNT; ++k) os << (k ? "," : "") << "\"" << fnames[k] << "\"";
@@ -1867,7 +1880,9 @@ bool launch_sweep(EkContext &ctx, const Sweep &s) {
     if (cfg.fast) {
         ek_cuda_check(ek_launch_sweep_fast(args, grid, cfg.T, cfg.smem, ctx.stream));
     } else {
-        ek_cuda_check(ek_launch_sweep(cfg.V, inline_prog, args, grid, cfg.T, cfg.smem, ctx.stream));
+        bool trig = false;          /* the general kernel's instantiation with the trigonometric operations */
+        for (const EkInstr &in : a.body) trig |= in.op >= DOP_TAN_F32 && in.op <= DOP_ATAN2R_F32;
+        ek_cuda_check(ek_launch_sweep(cfg.V, inline_prog, trig, args, grid, cfg.T, cfg.smem, ctx.stream));
     }
     if (ctx.timing) {
         ek_cuda_check(cudaEventRecord(ctx.ev_stop, ctx.stream));

@@ -133,7 +133,10 @@ struct EkInstr {
     X(RACC) X(RFIN) \
     /* init/fini helpers for privatised scatter_add bins and staged gather tables \
        (imm = descriptor index in the uniform pool; SMEM_ZERO: dst = 1 for float bins, which start at -0.0) */ \
-    X(SMEM_ZERO) X(SMEM_LOAD_TABLE) X(SMEM_FLUSH_ADD_F32) X(SMEM_FLUSH_ADD_I32)
+    X(SMEM_ZERO) X(SMEM_LOAD_TABLE) X(SMEM_FLUSH_ADD_F32) X(SMEM_FLUSH_ADD_I32) \
+    /* f32 trigonometric functions of array_math.h (ek_math.cuh), numbered last so that the operations above keep their \
+       numbers (ek_sweep_kernel<V, INLINE, false> carries none of them); ATAN2: R = y, B = x, ATAN2R: R = x, B = y */ \
+    X(TAN_F32) X(COT_F32) X(ASIN_F32) X(ACOS_F32) X(ATAN_F32) X(ATAN2_F32) X(ATAN2R_F32)
 
 enum EkDop : uint16_t {
 #define X(n) DOP_##n,
@@ -190,6 +193,17 @@ enum EkDop : uint16_t {
    of an output (numbered last, so that the operations of ek_fast_kernel keep their numbers) */
 #define EK_FOPS16(X) X(LD_F16) X(ST_F16)
 
+/* tan, cot, asin, acos, atan and atan2, in the bodies that the trig instantiations of ek_fast_kernel run (numbered after
+   the Float16 operations).  ATAN2 / ATAN2R: the accumulator is y / x; _U: the other operand is uniform-pool word b */
+#define EK_FOPST(X) X(TAN_F32) X(COT_F32) X(ASIN_F32) X(ACOS_F32) X(ATAN_F32) \
+                    X(ATAN2_F32) X(ATAN2_F32_U) X(ATAN2R_F32) X(ATAN2R_F32_U)
+
+/* feature bits of the ek_fast_kernel instantiations: the launcher runs the smallest one whose operations cover the
+   lowered body */
+#define EK_FX_F16  1u     /* FOP_LD_F16, FOP_ST_F16 */
+#define EK_FX_TRIG 2u     /* EK_FOPST */
+#define EK_FX_ALL  (EK_FX_F16 | EK_FX_TRIG)
+
 enum EkFop : uint16_t {
     FOP_NOP,
 #define X(n) FOP_##n, FOP_##n##_U,
@@ -199,9 +213,21 @@ enum EkFop : uint16_t {
     EK_FOPS1(X)
     EK_FOPS0(X)
     EK_FOPS16(X)
+    EK_FOPST(X)
 #undef X
     FOP__COUNT
 };
+
+/* the operation sets (EK_FX_*) that a lowered body uses: the instantiation of ek_fast_kernel that runs it */
+static inline uint32_t ek_fast_ext(const EkInstr *body, uint32_t n) {
+    uint32_t ext = 0;
+    for (uint32_t pc = 0; pc < n; ++pc) {
+        const uint32_t op = body[pc].op;
+        if (op == FOP_LD_F16 || op == FOP_ST_F16) ext |= EK_FX_F16;
+        else if (op >= FOP_TAN_F32 && op < FOP__COUNT) ext |= EK_FX_TRIG;
+    }
+    return ext;
+}
 
 /* ---- launch arguments (passed by value as a __grid_constant__ kernel parameter) ---- */
 #define EK_MAX_STAGED   16      /* staged (TMA) input arrays per sweep                  */

@@ -120,6 +120,96 @@ __device__ __forceinline__ float log_f32(float x) {
     return valid ? r : fbits(0xffffffffu);
 }
 
+/* ---------------- tan, cot, asin, acos, atan, atan2 ----------------
+   The single precision branches of array_math.h, restated operation for operation as the reference's generic body
+   records them on this backend (one node per primitive): separate mul / sub roundings, the same fmadd Estrin groupings,
+   cvttps2dq truncation, select, bit operations, and the correctly rounded rcp / division of DESIGN.md §4.  A result
+   is therefore bit-identical to the traced form, NaNs included.  Constants that the reference writes as double
+   literals are rounded to float once, as Scalar(c) does. */
+
+/* min/max with the x86 vminps/vmaxps operand rule of the CPU path
+   (array_avx.h min_/max_: second operand returned when either is NaN) */
+__device__ __forceinline__ float min_x86(float a, float b) { return a < b ? a : b; }
+__device__ __forceinline__ float max_x86(float a, float b) { return a > b ? a : b; }
+
+/* array_math.h:39-45 */
+__device__ __forceinline__ float poly4(float x, float c0, float c1, float c2, float c3, float c4) {
+    float x2 = fmul(x, x), x4 = fmul(x2, x2);
+    return ffma(x2, ffma(x, c3, c2), fadd(ffma(x, c1, c0), fmul(c4, x4)));
+}
+/* array_math.h:56-63 */
+__device__ __forceinline__ float poly6(float x, float c0, float c1, float c2, float c3, float c4, float c5, float c6) {
+    float x2 = fmul(x, x), x4 = fmul(x2, x2);
+    return ffma(x4, ffma(x2, c6, ffma(x, c5, c4)), ffma(x2, ffma(x, c3, c2), ffma(x, c1, c0)));
+}
+
+/* array_math.h:369-442 tancot_approx<Tan>, single precision branch (tan :466-468, cot :470-472) */
+template <bool Tan>
+__device__ __forceinline__ float tancot_f32(float x) {
+    float xa = fabsf(x);
+    int32_t j = cvtt_f32_i32(fmul(xa, (float) 1.2732395447351626862));
+    j = (j + 1) & ~1;
+    float y = __int2float_rn(j);
+    y = fsub(fsub(fsub(xa, fmul(y, (float) 0.78515625)), fmul(y, (float) 2.4187564849853515625e-4)),
+             fmul(y, (float) 3.77489497744594108e-8));
+    float z = fmul(y, y);
+    if (xa == __int_as_float(0x7f800000)) z = fbits(0xffffffffu);         /* z |= eq(xa, inf) */
+    float r = poly5(z, (float) 3.33331568548e-1, (float) 1.33387994085e-1, (float) 5.34112807005e-2,
+                       (float) 2.44301354525e-2, (float) 3.11992232697e-3, (float) 9.38540185543e-3);
+    r = ffma(r, fmul(z, y), y);
+    if (xa < (float) 1e-4) r = y;
+    const bool recip = Tan ? (j & 2) != 0 : (j & 2) == 0;
+    if (recip) r = __frcp_rn(r);
+    return fbits(ubits(r) ^ ((((uint32_t) j << 30) ^ ubits(x)) & 0x80000000u));   /* mulsign(r, sign) */
+}
+__device__ __forceinline__ float tan_f32(float x) { return tancot_f32<true>(x); }
+__device__ __forceinline__ float cot_f32(float x) { return tancot_f32<false>(x); }
+
+/* the shared part of array_math.h:493-508 (asin) and :570-585 (acos): returns z1, sets big = |x| > 0.5 */
+__device__ __forceinline__ float asincos_core(float x, float c0, bool &big) {
+    float xa = fabsf(x), x2 = fmul(x, x);
+    big = xa > 0.5f;
+    float x1 = fmul(0.5f, fsub(1.f, xa));
+    float x3 = big ? x1 : x2;
+    float x4 = big ? __fsqrt_rn(x1) : xa;
+    float z1 = poly4(x3, c0, 7.4953002686e-2f, 4.5470025998e-2f, 2.4181311049e-2f, 4.2163199048e-2f);
+    return ffma(z1, fmul(x3, x4), x4);
+}
+/* array_math.h:474-553 asin, single precision branch; copysign(r, x) = |r| | (x & sign) (array_router.h:398) */
+__device__ __forceinline__ float asin_f32(float x) {
+    bool big;
+    float z1 = asincos_core(x, 1.6666752422e-1f, big);
+    float r = big ? fsub((float) 1.57079632679489661923, fadd(z1, z1)) : z1;
+    return fbits((ubits(r) & 0x7fffffffu) | (ubits(x) & 0x80000000u));
+}
+/* array_math.h:555-590 acos, single precision branch */
+__device__ __forceinline__ float acos_f32(float x) {
+    bool big;
+    float z1 = asincos_core(x, 1.666675242e-1f, big);
+    float z2 = fadd(z1, z1);
+    if (x < 0.f) z2 = fsub((float) 3.14159265358979323846, z2);
+    float z3 = fsub((float) 1.57079632679489661923, fbits((ubits(z1) & 0x7fffffffu) | (ubits(x) & 0x80000000u)));
+    return big ? z2 : z3;
+}
+/* array_math.h:603-664 atan2(y, x), single precision branch.  min / max are the backend's (x86 operand rule),
+   1 / max is a correctly rounded division, and r &= neq(max, 0) selects +0. */
+__device__ __forceinline__ float atan2_f32(float y, float x) {
+    float abs_x = fabsf(x), abs_y = fabsf(y);
+    float min_val = min_x86(abs_y, abs_x), max_val = max_x86(abs_x, abs_y);
+    float scaled_min = fmul(min_val, __fdiv_rn(1.f, max_val));
+    float z = fmul(scaled_min, scaled_min);
+    float t = poly6(z, (float) 0.99999934166683966009, (float) -0.33326497518773606976, (float) +0.19881342388439013552,
+                       (float) -0.13486708938456973185, (float) +0.083863120428809689910, (float) -0.037006525670417265220,
+                       (float) 0.0078613793713198150252);
+    t = fmul(t, scaled_min);
+    if (abs_y > abs_x) t = fsub((float) 1.57079632679489661923, t);
+    if (x < 0.f) t = fsub((float) 3.14159265358979323846, t);
+    float r = y < 0.f ? fbits(ubits(t) ^ 0x80000000u) : t;
+    return max_val != 0.f ? r : 0.f;
+}
+/* array_math.h:666-668: atan(x) = atan2(x, 1) */
+__device__ __forceinline__ float atan_f32(float x) { return atan2_f32(x, 1.f); }
+
 /* ---------------- two elements at a time ----------------
    The sweep kernels evaluate exp / sin / cos on pairs of elements: the two independent dependency chains give
    ptxas instruction-level parallelism to interleave.  sm_90 has no packed fp32 arithmetic, so every pair
@@ -308,9 +398,7 @@ __device__ __forceinline__ double fma_nz(double a, double b, double c) {
 }
 
 /* min/max with the x86 vminps/vmaxps operand rule of the CPU path
-   (array_avx.h min_/max_: second operand returned when either is NaN) */
-__device__ __forceinline__ float min_x86(float a, float b) { return a < b ? a : b; }
-__device__ __forceinline__ float max_x86(float a, float b) { return a > b ? a : b; }
+   (array_avx.h min_/max_: second operand returned when either is NaN); float: above atan2_f32 */
 __device__ __forceinline__ double min_x86(double a, double b) { return a < b ? a : b; }
 __device__ __forceinline__ double max_x86(double a, double b) { return a > b ? a : b; }
 

@@ -51,7 +51,8 @@ const char *ek_op_name(ek_op op) {
         "exp", "log", "sin", "cos", "floor", "ceil", "round", "trunc", "floor2int", "ceil2int", "not",
         "popc", "clz", "ctz", "add", "sub", "mul", "mulhi", "div", "mod", "min", "max", "shl", "shr",
         "and", "or", "xor", "gt", "ge", "lt", "le", "eq", "ne", "mul_nz", "fma", "select", "fma_nz",
-        "gather", "scatter", "scatter_add", "hsum", "hprod", "hmax", "hmin", "all", "any", "count", "printf" };
+        "gather", "scatter", "scatter_add", "hsum", "hprod", "hmax", "hmin", "all", "any", "count", "printf",
+        "tan", "cot", "asin", "acos", "atan", "atan2" };
     return (unsigned) op < EK_OP__COUNT ? names[op] : "?";
 }
 
@@ -461,8 +462,8 @@ int ek_fetch_element(void *dst, uint32_t index, size_t offset, size_t size) {
 /* ------------------------------------------------------------------ trace append (jit.cu:701-861) */
 static int op_arity(ek_op op) {
     if (op == EK_OP_LITERAL || op == EK_OP_INDEX) return 0;
-    if (op >= EK_OP_MOV && op <= EK_OP_CTZ) return 1;
-    if (op >= EK_OP_ADD && op <= EK_OP_MUL_NZ) return 2;
+    if (ek_op_unary(op)) return 1;
+    if (ek_op_binary(op)) return 2;
     if (op == EK_OP_FMA || op == EK_OP_SELECT || op == EK_OP_FMA_NZ) return 3;
     if (op == EK_OP_GATHER || op == EK_OP_SCATTER || op == EK_OP_SCATTER_ADD) return 3;
     if (op >= EK_OP_HSUM && op <= EK_OP_COUNT) return 1;

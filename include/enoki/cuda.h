@@ -214,6 +214,17 @@ struct CUDAArray : ArrayBase<value_t<Value>, CUDAArray<Value>> {
     std::pair<CUDAArray, CUDAArray> sincos_() const { return { sin_(), cos_() }; }
     CUDAArray rcp_() const { return un_(EK_OP_RCP); }
     CUDAArray rsqrt_() const { return un_(EK_OP_RSQRT); }
+    /// tan/cot/asin/acos/atan/atan2: single opcodes for Float32 that compute, bit for bit, what array_math.h's
+    /// generic bodies (array_math.h:369-668) would record op by op.  array_math.h prefers these members when they
+    /// exist; for CUDAArray<double> and integer arrays they do not, and those keep the traced bodies.
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray tan_() const { return un_(EK_OP_TAN); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray cot_() const { return un_(EK_OP_COT); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray asin_() const { return un_(EK_OP_ASIN); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray acos_() const { return un_(EK_OP_ACOS); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray atan_() const { return un_(EK_OP_ATAN); }
+    /// atan2(*this, x): *this is y
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0>
+    CUDAArray atan2_(const CUDAArray &x) const { return bin_(EK_OP_ATAN2, x); }
     CUDAArray floor_() const { return un_(EK_OP_FLOOR); }
     CUDAArray ceil_() const { return un_(EK_OP_CEIL); }
     CUDAArray round_() const { return un_(EK_OP_ROUND); }

@@ -117,6 +117,14 @@ typedef enum ek_op {
     EK_OP_ALL, EK_OP_ANY, EK_OP_COUNT,
     /* print node of ek_trace_printf() (jit.cu:863-916); not accepted by ek_trace_append()                  */
     EK_OP_PRINTF,
+    /* Float32 only (other types are refused); appended so that no opcode above changes its number.  Each is ONE node
+       that evaluates the single precision branch of array_math.h bit for bit as its traced form would              */
+    EK_OP_TAN,         /* array_math.h:369-468  tancot_approx<true>                         */
+    EK_OP_COT,         /* array_math.h:369-472  tancot_approx<false>                        */
+    EK_OP_ASIN,        /* array_math.h:474-553 */
+    EK_OP_ACOS,        /* array_math.h:555-601 */
+    EK_OP_ATAN,        /* array_math.h:666-668  atan2(x, 1)                                 */
+    EK_OP_ATAN2,       /* array_math.h:603-664  operands (y, x), like atan2(y, x)           */
     EK_OP__COUNT
 } ek_op;
 
