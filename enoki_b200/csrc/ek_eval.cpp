@@ -112,6 +112,18 @@ int norm_op(ek_type t) {
     }
 }
 
+/* the 32-bit register word of a value of type t with the given bits: a narrow value sign- or zero-extended from the
+   type's width (as the sweep kernels hold it and load scalars), whatever lies above those bits */
+uint32_t register_word(ek_type t, uint64_t bits) {
+    switch (t) {
+        case EK_INT8: return (uint32_t) (int32_t) (int8_t) bits;
+        case EK_UINT8: return (uint32_t) (uint8_t) bits;
+        case EK_INT16: return (uint32_t) (int32_t) (int16_t) bits;
+        case EK_UINT16: case EK_FLOAT16: return (uint32_t) (uint16_t) bits;
+        default: return (uint32_t) bits;
+    }
+}
+
 #define SEL(f32, f64, i32, u32, i64, u64) \
     (c == C_F32 ? (f32) : c == C_F64 ? (f64) : c == C_I32 ? (i32) : c == C_U32 ? (u32) : c == C_I64 ? (i64) : (u64))
 
@@ -529,7 +541,7 @@ struct Assembler {
                 }
             } else if (v.op == EK_OP_LITERAL) {
                 if (ek_is_64(v.type)) loc[idx] = { Loc::UNI, uni_lit(lit_pair(v.imm)) };
-                else loc[idx] = { Loc::UNI, uni_lit(lit_word((uint32_t) v.imm)) };
+                else loc[idx] = { Loc::UNI, uni_lit(lit_word(register_word(v.type, v.imm))) };
             }
         }
         out.n_in_units = unit;
@@ -862,9 +874,10 @@ struct Assembler {
             case EK_OP_AND: case EK_OP_OR: {
                 ek_type bt = var(d1).type;
                 if (t != EK_BOOL && bt == EK_BOOL) {
-                    /* value & mask = select(mask, value, 0); value | mask = select(mask, ~0, value) (cuda.h:545-572) */
+                    /* value & mask = select(mask, value, 0); value | mask = select(mask, ~0, value) (cuda.h:545-572), ~0 as the
+                       type's register holds it (0xff for UInt8) */
                     uint16_t k = is64 ? uni_lit(lit_pair(op == EK_OP_AND ? 0ull : ~0ull))
-                                      : uni_lit(lit_word(op == EK_OP_AND ? 0u : 0xffffffffu));
+                                      : uni_lit(lit_word(op == EK_OP_AND ? 0u : register_word(t, ~0ull)));
                     int p = acc_at(d0, d1, 0);
                     if (p < 0) { ensure_acc(d0); p = 0; }
                     if (op == EK_OP_AND) {

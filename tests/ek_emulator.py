@@ -13,6 +13,7 @@ OP_NONE = 0xFFFF
 NEG_ZERO = 0x80000000                      # bits of -0.0f, the start value of float scatter_add bins
 SZ = ctypes.c_size_t
 T_FLOAT32, T_INT32, T_UINT32, T_BOOL, T_INT64, T_UINT64, T_FLOAT64 = 10, 5, 6, 12, 7, 8, 11
+T_INT8, T_UINT8 = 1, 2
 
 
 class Unsupported(Exception):
@@ -555,6 +556,9 @@ class Emulator:
                 elif name == "SHL_32": R = np.where(B >= 32, np.uint32(0), R << (B & np.uint32(31)))
                 elif name == "SHR_U32": R = np.where(B >= 32, np.uint32(0), R >> (B & np.uint32(31)))
                 elif name == "SHR_I32": R = (R.view(np.int32) >> np.minimum(B, np.uint32(31)).astype(np.int32)).view(np.uint32)
+                elif name == "SHLR_32": R = np.where(R >= 32, np.uint32(0), B << (R & np.uint32(31)))
+                elif name == "SHRR_U32": R = np.where(R >= 32, np.uint32(0), B >> (R & np.uint32(31)))
+                elif name == "SHRR_I32": R = (B.view(np.int32) >> np.minimum(R, np.uint32(31)).astype(np.int32)).view(np.uint32)
                 elif name in ("MIN_U32", "MAX_U32"): R = (np.minimum if name == "MIN_U32" else np.maximum)(R, B)
                 elif name in ("MIN_I32", "MAX_I32"): R = (np.minimum if name == "MIN_I32" else np.maximum)(R.view(np.int32), B.view(np.int32)).view(np.uint32)
                 elif name in ("LT_U32", "LE_U32", "GT_U32", "GE_U32"):

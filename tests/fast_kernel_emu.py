@@ -8,7 +8,7 @@ import subprocess
 
 import numpy as np
 
-from ek_emulator import Emulator, T_BOOL, T_FLOAT32, T_INT32, T_UINT32
+from ek_emulator import Emulator, T_BOOL, T_FLOAT32, T_INT32, T_INT8, T_UINT32, T_UINT8
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 _lib = None
@@ -26,7 +26,7 @@ def emu_lib():
     return _lib
 
 
-_DT = {T_FLOAT32: np.float32, T_INT32: np.int32, T_UINT32: np.uint32, T_BOOL: np.uint8}
+_DT = {T_FLOAT32: np.float32, T_INT32: np.int32, T_UINT32: np.uint32, T_BOOL: np.uint8, T_INT8: np.int8, T_UINT8: np.uint8}
 
 
 class FastKernelEmulator(Emulator):

@@ -62,7 +62,7 @@ def test_ops64_on_the_emulator(ek, oracle, clean, program_form, tname, form):
     ops = cv.ops64(tname, form)
     for n in (1, 4097):
         for k in range(0, len(ops), 8):
-            _run(ek, oracle, lambda put: cv.ops64_case(ek, put, tname, ops[k:k + 8], n, form, seed=n + k))
+            _run(ek, oracle, lambda put: cv.ops_case(ek, put, tname, ops[k:k + 8], n, form, seed=n + k))
 
 
 def test_float_to_uint32_on_the_host_compiled_kernel(ek, oracle, clean, program_form):
