@@ -23,7 +23,7 @@ _OPS = ["INVALID", "LITERAL", "INDEX", "MOV", "CVT", "BITCAST", "NEG", "ABS", "S
         "POPC", "CLZ", "CTZ", "ADD", "SUB", "MUL", "MULHI", "DIV", "MOD", "MIN", "MAX", "SHL", "SHR",
         "AND", "OR", "XOR", "GT", "GE", "LT", "LE", "EQ", "NE", "MUL_NZ", "FMA", "SELECT", "FMA_NZ",
         "GATHER", "SCATTER", "SCATTER_ADD", "HSUM", "HPROD", "HMAX", "HMIN", "ALL", "ANY", "COUNT", "PRINTF",
-        "TAN", "COT", "ASIN", "ACOS", "ATAN", "ATAN2"]
+        "TAN", "COT", "ASIN", "ACOS", "ATAN", "ATAN2", "SINH", "COSH", "TANH", "ASINH", "ACOSH", "ATANH", "CBRT"]
 OP = {n: i for i, n in enumerate(_OPS)}
 
 _NP = {EK_INT8: np.int8, EK_UINT8: np.uint8, EK_INT16: np.int16, EK_UINT16: np.uint16,
@@ -246,6 +246,12 @@ popcnt, lzcnt, tzcnt = (_unary(o) for o in ("POPC", "CLZ", "CTZ"))
 abs_ = _unary("ABS")
 # Float32 only: one node each, bit for bit the single precision branch of array_math.h (DESIGN.md 4)
 tan, cot, asin, acos, atan = (_unary(o) for o in ("TAN", "COT", "ASIN", "ACOS", "ATAN"))
+sinh, cosh, tanh, asinh, acosh, atanh, cbrt = (_unary(o) for o in ("SINH", "COSH", "TANH", "ASINH", "ACOSH", "ATANH", "CBRT"))
+
+
+def sincosh(x):
+    """(sinh(x), cosh(x)): array_math.h:1067-1127 records the same operations as the two functions"""
+    return sinh(x), cosh(x)
 
 
 def atan2(y, x):

@@ -126,6 +126,7 @@ def _unary(label, f, dfdx):
 def _build():
     from . import sin as _sin, cos as _cos, exp as _exp, log as _log, sqrt as _sqrt, rcp as _rcp, Float32, UInt32, reinterpret
     from . import tan as _tan, cot as _cot, asin as _asin, acos as _acos, atan as _atan, rsqrt as _rsqrt
+    from . import sinh as _sinh, cosh as _cosh, tanh as _tanh, asinh as _asinh, acosh as _acosh, atanh as _atanh, cbrt as _cbrt
 
     def _sign(a):
         # sign(a) = (sign_mask & a) | 1.0 (array_router.h:372): -1 at -0.0 and at NaNs with the sign bit set
@@ -153,6 +154,18 @@ def _build():
     g["asin"] = _unary("asin", _asin, lambda a, r: _rsqrt(1.0 - a * a))         # autodiff.h:582-592
     g["acos"] = _unary("acos", _acos, lambda a, r: -_rsqrt(1.0 - a * a))        # autodiff.h:594-604
     g["atan"] = _unary("atan", _atan, lambda a, r: _rcp(1.0 + a * a))           # autodiff.h:606-616
+
+    def _sqr_sech(a):
+        s = _rcp(_cosh(a))
+        return s * s
+
+    g["sinh"] = _unary("sinh", _sinh, lambda a, r: _cosh(a))                    # autodiff.h:635-645
+    g["cosh"] = _unary("cosh", _cosh, lambda a, r: _sinh(a))                    # autodiff.h:647-657
+    g["tanh"] = _unary("tanh", _tanh, lambda a, r: _sqr_sech(a))                # autodiff.h:685-696: sqr(sech(a))
+    g["asinh"] = _unary("asinh", _asinh, lambda a, r: _rsqrt(1.0 + a * a))      # autodiff.h:698-708
+    g["acosh"] = _unary("acosh", _acosh, lambda a, r: _rsqrt(a * a - 1.0))      # autodiff.h:710-720
+    g["atanh"] = _unary("atanh", _atanh, lambda a, r: _rcp(1.0 - a * a))        # autodiff.h:722-732
+    g["cbrt"] = _unary("cbrt", _cbrt, lambda a, r: 1.0 / (3.0 * (r * r)))      # autodiff.h:366-377
     return g
 
 
@@ -178,6 +191,13 @@ def cot(x): return _op("cot")(x)
 def asin(x): return _op("asin")(x)
 def acos(x): return _op("acos")(x)
 def atan(x): return _op("atan")(x)
+def sinh(x): return _op("sinh")(x)
+def cosh(x): return _op("cosh")(x)
+def tanh(x): return _op("tanh")(x)
+def asinh(x): return _op("asinh")(x)
+def acosh(x): return _op("acosh")(x)
+def atanh(x): return _op("atanh")(x)
+def cbrt(x): return _op("cbrt")(x)
 
 
 def atan2(y, x):

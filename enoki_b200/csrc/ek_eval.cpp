@@ -148,6 +148,13 @@ int pick_op(ek_op op, ek_type vt, ek_type at /* operand type */) {
         case EK_OP_ACOS:  return SEL(DOP_ACOS_F32, -1, -1, -1, -1, -1);
         case EK_OP_ATAN:  return SEL(DOP_ATAN_F32, -1, -1, -1, -1, -1);
         case EK_OP_ATAN2: return SEL(DOP_ATAN2_F32, -1, -1, -1, -1, -1);
+        case EK_OP_SINH:  return SEL(DOP_SINH_F32, -1, -1, -1, -1, -1);
+        case EK_OP_COSH:  return SEL(DOP_COSH_F32, -1, -1, -1, -1, -1);
+        case EK_OP_TANH:  return SEL(DOP_TANH_F32, -1, -1, -1, -1, -1);
+        case EK_OP_ASINH: return SEL(DOP_ASINH_F32, -1, -1, -1, -1, -1);
+        case EK_OP_ACOSH: return SEL(DOP_ACOSH_F32, -1, -1, -1, -1, -1);
+        case EK_OP_ATANH: return SEL(DOP_ATANH_F32, -1, -1, -1, -1, -1);
+        case EK_OP_CBRT:  return SEL(DOP_CBRT_F32, -1, -1, -1, -1, -1);
         case EK_OP_FLOOR: return SEL(DOP_FLOOR_F32, DOP_FLOOR_F64, DOP_LOAD_32, DOP_LOAD_32, DOP_LOAD_64, DOP_LOAD_64);
         case EK_OP_CEIL:  return SEL(DOP_CEIL_F32, DOP_CEIL_F64, DOP_LOAD_32, DOP_LOAD_32, DOP_LOAD_64, DOP_LOAD_64);
         case EK_OP_ROUND: return SEL(DOP_ROUND_F32, DOP_ROUND_F64, DOP_LOAD_32, DOP_LOAD_32, DOP_LOAD_64, DOP_LOAD_64);
@@ -1003,7 +1010,7 @@ struct Assembler {
 
     /* does the instruction leave its imm field unused (so that EKF_STG can use it)? */
     static bool imm_free(int op) {
-        if (op >= DOP_TAN_F32 && op <= DOP_ATAN2R_F32) return true;
+        if (ek_dop_ext(op)) return true;
         if (op >= DOP_CVT_F32_I32 && op <= DOP_CVT_64_32) return false;
         if (op >= DOP_LD_U8) return false;          /* loads, stores, gathers, scatters, reductions, smem helpers */
         return true;
@@ -1070,6 +1077,10 @@ struct Assembler {
             switch (in.op) { case DOP_SIN_F32: case DOP_COS_F32: case DOP_EXP_F32: case DOP_LOG_F32: return 8.0;
                              case DOP_TAN_F32: case DOP_COT_F32: return 12.0;
                              case DOP_ASIN_F32: case DOP_ACOS_F32: case DOP_ATAN_F32: case DOP_ATAN2_F32: case DOP_ATAN2R_F32: return 10.0;
+                             case DOP_COSH_F32: return 10.0;
+                             case DOP_SINH_F32: case DOP_TANH_F32: case DOP_ATANH_F32: return 12.0;
+                             case DOP_ASINH_F32: case DOP_ACOSH_F32: return 14.0;
+                             case DOP_CBRT_F32: return 16.0;
                              case DOP_SQRT_F32: case DOP_DIV_F32: case DOP_RCP_F32: case DOP_RSQRT_F32: return 3.0; default: return 1.0; } };
         double total_w = 0; for (const EkInstr &in : out.body) total_w += weight(in);
         double acc_w = 0;
@@ -1287,6 +1298,7 @@ int fop_of(int dop) {
         X(SCATTER_ADD_F32_SMEM) X(SCATTER_ADD_I32_SMEM) X(RACC)
         EK_FOPS0(X)
         X(TAN_F32) X(COT_F32) X(ASIN_F32) X(ACOS_F32) X(ATAN_F32) X(ATAN2_F32) X(ATAN2R_F32)
+        X(SINH_F32) X(COSH_F32) X(TANH_F32) X(ASINH_F32) X(ACOSH_F32) X(ATANH_F32) X(CBRT_F32)
 #undef X
         case DOP_LOAD_32: return FOP_LOAD;
         default: return -1;
@@ -1791,7 +1803,7 @@ void write_program_json(std::ostream &os, const EkContext &ctx, const std::vecto
             EK_FOPS2(X)
 #undef X
 #define X(n) #n,
-            EK_FOPS1(X) EK_FOPS0(X) EK_FOPS16(X) EK_FOPST(X)
+            EK_FOPS1(X) EK_FOPS0(X) EK_FOPS16(X) EK_FOPST(X) EK_FOPSH(X)
 #undef X
         };
         for (int k = 0; k < FOP__COUNT; ++k) os << (k ? "," : "") << "\"" << fnames[k] << "\"";
@@ -1893,8 +1905,8 @@ bool launch_sweep(EkContext &ctx, const Sweep &s) {
     if (cfg.fast) {
         ek_cuda_check(ek_launch_sweep_fast(args, grid, cfg.T, cfg.smem, ctx.stream));
     } else {
-        bool trig = false;          /* the general kernel's instantiation with the trigonometric operations */
-        for (const EkInstr &in : a.body) trig |= in.op >= DOP_TAN_F32 && in.op <= DOP_ATAN2R_F32;
+        bool trig = false;          /* the general kernel's instantiation with the trigonometric and hyperbolic operations */
+        for (const EkInstr &in : a.body) trig |= ek_dop_ext(in.op);
         ek_cuda_check(ek_launch_sweep(cfg.V, inline_prog, trig, args, grid, cfg.T, cfg.smem, ctx.stream));
     }
     if (ctx.timing) {

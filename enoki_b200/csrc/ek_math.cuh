@@ -210,6 +210,112 @@ __device__ __forceinline__ float atan2_f32(float y, float x) {
 /* array_math.h:666-668: atan(x) = atan2(x, 1) */
 __device__ __forceinline__ float atan_f32(float x) { return atan2_f32(x, 1.f); }
 
+/* ---------------- sinh, cosh, tanh, asinh, acosh, atanh, cbrt ----------------
+   Restated like the trigonometric functions above: each is the operation sequence of the traced single precision body,
+   with this backend's exp_f32 / log_f32, the correctly rounded rcp, sqrt and division, and the mask operations as the
+   bit operations the backend records for them: value & ~mask gives +0 where the mask is set, value | mask all ones. */
+
+/* array_math.h:31-37 */
+__device__ __forceinline__ float poly3(float x, float c0, float c1, float c2, float c3) {
+    float x2 = fmul(x, x);
+    return ffma(x2, ffma(x, c3, c2), ffma(x, c1, c0));
+}
+/* copysign(r, x) = |r| | (x & sign) (array_router.h:398) */
+__device__ __forceinline__ float copysign_bits(float r, float x) {
+    return fbits((ubits(r) & 0x7fffffffu) | (ubits(x) & 0x80000000u));
+}
+
+/* array_math.h:1067-1127 sincosh, which is sinh :997-1046 and cosh :1048-1065 computed together: both start from
+   exp0 = exp(x), exp1 = rcp(exp0) */
+template <bool Sinh, bool Cosh>
+__device__ __forceinline__ void sincosh_f32(float x, float &s_out, float &c_out) {
+    float exp0 = exp_f32(x), exp1 = __frcp_rn(exp0);
+    if (Sinh) {
+        float x2 = fmul(x, x);
+        float r_small = ffma(poly2(x2, (float) 1.66667160211e-1, (float) 8.33028376239e-3, (float) 2.03721912945e-4),
+                             fmul(x2, x), x);
+        float r_big = fmul(fsub(exp0, exp1), 0.5f);
+        s_out = fabsf(x) > 1.f ? r_big : r_small;
+    }
+    if (Cosh) c_out = fmul(fadd(exp0, exp1), 0.5f);
+}
+__device__ __forceinline__ float sinh_f32(float x) { float s, c; sincosh_f32<true, false>(x, s, c); return s; }
+__device__ __forceinline__ float cosh_f32(float x) { float s, c; sincosh_f32<false, true>(x, s, c); return c; }
+
+/* array_math.h:1129-1179 tanh, single precision branch */
+__device__ __forceinline__ float tanh_f32(float x) {
+    float x2 = fmul(x, x);
+    float r_small = poly4(x2, (float) -3.33332819422e-1, (float) 1.33314422036e-1, (float) -5.37397155531e-2,
+                              (float) 2.06390887954e-2, (float) -5.70498872745e-3);
+    r_small = ffma(r_small, fmul(x2, x), x);
+    float e = exp_f32(fadd(x, x)), e2 = __frcp_rn(fadd(e, 1.f));
+    float r_big = fsub(1.f, fadd(e2, e2));
+    return fabsf(x) >= 0.625f ? r_big : r_small;
+}
+
+/* array_math.h:1185-1237 asinh, single precision branch */
+__device__ __forceinline__ float asinh_f32(float x) {
+    float x2 = fmul(x, x), xa = fabsf(x);
+    bool big = xa >= (float) 0.51, huge = xa >= (float) 1e10;
+    float r_small = poly3(x2, (float) -1.6666288134e-1, (float) 7.4847586088e-2, (float) -4.2699340972e-2,
+                              (float) 2.0122003309e-2);
+    r_small = ffma(r_small, fmul(x2, x), x);
+    float r_big = log_f32(fadd(huge ? 0.f : __fsqrt_rn(fadd(x2, 1.f)), xa));     /* sqrt(x2 + 1) & ~mask_huge */
+    if (huge) r_big = fadd(r_big, (float) 0.693147180559945309417);               /* r_big[mask_huge] += M_LN2 */
+    r_big = copysign_bits(r_big, x);
+    return big ? r_big : r_small;
+}
+
+/* array_math.h:1239-1293 acosh, single precision branch.  fmsub(x, x, 1) is fma(x, x, -1). */
+__device__ __forceinline__ float acosh_f32(float x) {
+    float x1 = fsub(x, 1.f);
+    bool big = x1 >= (float) 0.49, huge = x1 >= (float) 1e10;
+    float r_small = poly4(x1, (float) 1.4142135263e+0, (float) -1.1784741703e-1, (float) 2.6454905019e-2,
+                              (float) -7.5272886713e-3, (float) 1.7596881071e-3);
+    r_small = fmul(__fsqrt_rn(x1), r_small);
+    if (x1 < 0.f) r_small = fbits(0xffffffffu);                                   /* r_small |= x1 < 0 */
+    float r_big = log_f32(fadd(huge ? 0.f : __fsqrt_rn(ffma(x, x, -1.f)), x));
+    if (huge) r_big = fadd(r_big, (float) 0.693147180559945309417);
+    return big ? r_big : r_small;
+}
+
+/* array_math.h:1295-1348 atanh, single precision branch */
+__device__ __forceinline__ float atanh_f32(float x) {
+    float xa = fabsf(x), x2 = fmul(x, x);
+    float r_small = poly4(x2, (float) 3.33337300303e-1, (float) 1.99782164500e-1, (float) 1.46691431730e-1,
+                              (float) 8.24370301058e-2, (float) 1.81740078349e-1);
+    r_small = ffma(r_small, fmul(x2, x), x);
+    float r_big = fmul(log_f32(__fdiv_rn(fadd(xa, 1.f), fsub(1.f, xa))), 0.5f);
+    r_big = copysign_bits(r_big, x);
+    return xa >= 0.5f ? r_big : r_small;
+}
+
+/* array_math.h:900-954 cbrt, single precision branch (one Newton step), with frexp :682-709 and ldexp :677-680.  frexp
+   treats 0 and denormals as normal numbers: cbrt(+-0) is +-0.337986261 and cbrt(1e-45) 1.2e-13, as on the CPU path. */
+__device__ __forceinline__ float cbrt_f32(float x) {
+    const float third = (float) (1.0 / 3.0);
+    float xa = fabsf(x);
+    uint32_t xi = ubits(xa), exponent_bits = xi & 0x7f800000u;
+    bool is_normal = exponent_bits != 0x7f800000u && xa != 0.f;
+    float xm = fbits(is_normal ? (xi & 0x807fffffu) | 0x3f000000u : xi);
+    float xe = fadd(__int2float_rn(is_normal ? (int32_t) (exponent_bits >> 23) - 0x7f : 0), 1.f);
+    float xea = fabsf(xe), xea1 = floorf(fmul(xea, third));
+    float rem = ffma(xea1, -3.f, xea);                                            /* fnmadd(xea1, 3, xea) */
+    xm = poly4(xm, (float) 0.40238979564544752126924, (float) 1.1399983354717293273738,
+                   (float) -0.95438224771509446525043, (float) 0.54664601366395524503440,
+                   (float) -0.13466110473359520655053);
+    /* CBRT2, CBRT4 and Scalar(1) / CBRT2, Scalar(1) / CBRT4, the latter two divided in float */
+    float f1 = xe >= 0.f ? fbits(0x3fa14518u) : fbits(0x3f4b2ff5u);
+    float f2 = xe >= 0.f ? fbits(0x3fcb2ff5u) : fbits(0x3f214518u);
+    float f = rem == 1.f ? f1 : f2;
+    if (rem != 0.f) xm = fmul(f, xm);                                             /* xm[neq(rem, 0)] *= f */
+    float e = fbits(ubits(xea1) ^ (ubits(xe) & 0x80000000u));                     /* mulsign(xea1, xe) */
+    float r = fmul(fbits(((uint32_t) cvtt_f32_i32(e) + 0x7fu) << 23), xm);        /* ldexp(xm, e) */
+    r = fbits(ubits(r) ^ (ubits(x) & 0x80000000u));                               /* mulsign(r, x) */
+    r = fsub(r, fmul(fsub(r, __fdiv_rn(x, fmul(r, r))), third));
+    return fabsf(x) < __int_as_float(0x7f800000) ? r : x;
+}
+
 /* ---------------- two elements at a time ----------------
    The sweep kernels evaluate exp / sin / cos on pairs of elements: the two independent dependency chains give
    ptxas instruction-level parallelism to interleave.  sm_90 has no packed fp32 arithmetic, so every pair

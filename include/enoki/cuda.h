@@ -225,6 +225,19 @@ struct CUDAArray : ArrayBase<value_t<Value>, CUDAArray<Value>> {
     /// atan2(*this, x): *this is y
     template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0>
     CUDAArray atan2_(const CUDAArray &x) const { return bin_(EK_OP_ATAN2, x); }
+    /// sinh/cosh/tanh/asinh/acosh/atanh/cbrt: the same for the hyperbolic functions and the cube root
+    /// (array_math.h:900-954,997-1348).  csch, sech and coth are rcp() of these.
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray sinh_() const { return un_(EK_OP_SINH); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray cosh_() const { return un_(EK_OP_COSH); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray tanh_() const { return un_(EK_OP_TANH); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray asinh_() const { return un_(EK_OP_ASINH); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray acosh_() const { return un_(EK_OP_ACOSH); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray atanh_() const { return un_(EK_OP_ATANH); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray cbrt_() const { return un_(EK_OP_CBRT); }
+    /// sincosh (array_math.h:1067-1127) records the same operations as sinh followed by cosh, so it is the pair of them
+    /// (DiffArray's sinh_ / cosh_ call it)
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0>
+    std::pair<CUDAArray, CUDAArray> sincosh_() const { return { sinh_(), cosh_() }; }
     CUDAArray floor_() const { return un_(EK_OP_FLOOR); }
     CUDAArray ceil_() const { return un_(EK_OP_CEIL); }
     CUDAArray round_() const { return un_(EK_OP_ROUND); }

@@ -125,6 +125,13 @@ typedef enum ek_op {
     EK_OP_ACOS,        /* array_math.h:555-601 */
     EK_OP_ATAN,        /* array_math.h:666-668  atan2(x, 1)                                 */
     EK_OP_ATAN2,       /* array_math.h:603-664  operands (y, x), like atan2(y, x)           */
+    EK_OP_SINH,        /* array_math.h:997-1046 */
+    EK_OP_COSH,        /* array_math.h:1048-1065 */
+    EK_OP_TANH,        /* array_math.h:1129-1179 */
+    EK_OP_ASINH,       /* array_math.h:1185-1237 */
+    EK_OP_ACOSH,       /* array_math.h:1239-1293 */
+    EK_OP_ATANH,       /* array_math.h:1295-1348 */
+    EK_OP_CBRT,        /* array_math.h:900-954  frexp :682-709, ldexp :677-680              */
     EK_OP__COUNT
 } ek_op;
 
