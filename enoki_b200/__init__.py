@@ -24,7 +24,10 @@ _OPS = ["INVALID", "LITERAL", "INDEX", "MOV", "CVT", "BITCAST", "NEG", "ABS", "S
         "AND", "OR", "XOR", "GT", "GE", "LT", "LE", "EQ", "NE", "MUL_NZ", "FMA", "SELECT", "FMA_NZ",
         "GATHER", "SCATTER", "SCATTER_ADD", "HSUM", "HPROD", "HMAX", "HMIN", "ALL", "ANY", "COUNT", "PRINTF",
         "TAN", "COT", "ASIN", "ACOS", "ATAN", "ATAN2", "SINH", "COSH", "TANH", "ASINH", "ACOSH", "ATANH", "CBRT"]
-OP = {n: i for i, n in enumerate(_OPS)}
+# special.h's functions, numbered after EK_OP_CBRT (include/enoki_b200.h) in a group of their own, like their sweep
+# operations (EK_FX_SPEC)
+_OPS_SPECIAL = ["ERF", "ERFC", "ERFINV", "LGAMMA", "TGAMMA"]
+OP = {n: i for i, n in enumerate(_OPS + _OPS_SPECIAL)}
 
 _NP = {EK_INT8: np.int8, EK_UINT8: np.uint8, EK_INT16: np.int16, EK_UINT16: np.uint16,
        EK_INT32: np.int32, EK_UINT32: np.uint32, EK_INT64: np.int64, EK_UINT64: np.uint64,
@@ -247,6 +250,8 @@ abs_ = _unary("ABS")
 # Float32 only: one node each, bit for bit the single precision branch of array_math.h (DESIGN.md 4)
 tan, cot, asin, acos, atan = (_unary(o) for o in ("TAN", "COT", "ASIN", "ACOS", "ATAN"))
 sinh, cosh, tanh, asinh, acosh, atanh, cbrt = (_unary(o) for o in ("SINH", "COSH", "TANH", "ASINH", "ACOSH", "ATANH", "CBRT"))
+# Float32 only: one node each, bit for bit the single precision branch of special.h (DESIGN.md 4)
+erf, erfc, erfinv, lgamma, tgamma = (_unary(o) for o in ("ERF", "ERFC", "ERFINV", "LGAMMA", "TGAMMA"))
 
 
 def sincosh(x):

@@ -127,6 +127,7 @@ def _build():
     from . import sin as _sin, cos as _cos, exp as _exp, log as _log, sqrt as _sqrt, rcp as _rcp, Float32, UInt32, reinterpret
     from . import tan as _tan, cot as _cot, asin as _asin, acos as _acos, atan as _atan, rsqrt as _rsqrt
     from . import sinh as _sinh, cosh as _cosh, tanh as _tanh, asinh as _asinh, acosh as _acosh, atanh as _atanh, cbrt as _cbrt
+    from . import erf as _erf, erfc as _erfc, erfinv as _erfinv
 
     def _sign(a):
         # sign(a) = (sign_mask & a) | 1.0 (array_router.h:372): -1 at -0.0 and at NaNs with the sign bit set
@@ -166,6 +167,12 @@ def _build():
     g["acosh"] = _unary("acosh", _acosh, lambda a, r: _rsqrt(a * a - 1.0))      # autodiff.h:710-720
     g["atanh"] = _unary("atanh", _atanh, lambda a, r: _rcp(1.0 - a * a))        # autodiff.h:722-732
     g["cbrt"] = _unary("cbrt", _cbrt, lambda a, r: 1.0 / (3.0 * (r * r)))      # autodiff.h:366-377
+
+    # autodiff.h has no weights for special.h's functions: these are the analytic derivatives
+    two_over_sqrt_pi, sqrt_pi_over_2 = 1.1283791670955126, 0.886226925452758
+    g["erf"] = _unary("erf", _erf, lambda a, r: two_over_sqrt_pi * _exp(-(a * a)))
+    g["erfc"] = _unary("erfc", _erfc, lambda a, r: -two_over_sqrt_pi * _exp(-(a * a)))
+    g["erfinv"] = _unary("erfinv", _erfinv, lambda a, r: sqrt_pi_over_2 * _exp(r * r))
     return g
 
 
@@ -198,6 +205,21 @@ def asinh(x): return _op("asinh")(x)
 def acosh(x): return _op("acosh")(x)
 def atanh(x): return _op("atanh")(x)
 def cbrt(x): return _op("cbrt")(x)
+
+
+def erf(x):
+    """erf(x); weight (2 / sqrt(pi)) * exp(-x * x)"""
+    return _op("erf")(x)
+
+
+def erfc(x):
+    """erfc(x); weight -(2 / sqrt(pi)) * exp(-x * x)"""
+    return _op("erfc")(x)
+
+
+def erfinv(x):
+    """erfinv(x); weight (sqrt(pi) / 2) * exp(r * r), where r = erfinv(x)"""
+    return _op("erfinv")(x)
 
 
 def atan2(y, x):

@@ -155,6 +155,11 @@ int pick_op(ek_op op, ek_type vt, ek_type at /* operand type */) {
         case EK_OP_ACOSH: return SEL(DOP_ACOSH_F32, -1, -1, -1, -1, -1);
         case EK_OP_ATANH: return SEL(DOP_ATANH_F32, -1, -1, -1, -1, -1);
         case EK_OP_CBRT:  return SEL(DOP_CBRT_F32, -1, -1, -1, -1, -1);
+        case EK_OP_ERF:    return SEL(DOP_ERF_F32, -1, -1, -1, -1, -1);
+        case EK_OP_ERFC:   return SEL(DOP_ERFC_F32, -1, -1, -1, -1, -1);
+        case EK_OP_ERFINV: return SEL(DOP_ERFINV_F32, -1, -1, -1, -1, -1);
+        case EK_OP_LGAMMA: return SEL(DOP_LGAMMA_F32, -1, -1, -1, -1, -1);
+        case EK_OP_TGAMMA: return SEL(DOP_TGAMMA_F32, -1, -1, -1, -1, -1);
         case EK_OP_FLOOR: return SEL(DOP_FLOOR_F32, DOP_FLOOR_F64, DOP_LOAD_32, DOP_LOAD_32, DOP_LOAD_64, DOP_LOAD_64);
         case EK_OP_CEIL:  return SEL(DOP_CEIL_F32, DOP_CEIL_F64, DOP_LOAD_32, DOP_LOAD_32, DOP_LOAD_64, DOP_LOAD_64);
         case EK_OP_ROUND: return SEL(DOP_ROUND_F32, DOP_ROUND_F64, DOP_LOAD_32, DOP_LOAD_32, DOP_LOAD_64, DOP_LOAD_64);
@@ -1081,6 +1086,8 @@ struct Assembler {
                              case DOP_SINH_F32: case DOP_TANH_F32: case DOP_ATANH_F32: return 12.0;
                              case DOP_ASINH_F32: case DOP_ACOSH_F32: return 14.0;
                              case DOP_CBRT_F32: return 16.0;
+                             case DOP_ERF_F32: case DOP_ERFC_F32: case DOP_ERFINV_F32: return 14.0;
+                             case DOP_LGAMMA_F32: case DOP_TGAMMA_F32: return 20.0;
                              case DOP_SQRT_F32: case DOP_DIV_F32: case DOP_RCP_F32: case DOP_RSQRT_F32: return 3.0; default: return 1.0; } };
         double total_w = 0; for (const EkInstr &in : out.body) total_w += weight(in);
         double acc_w = 0;
@@ -1299,6 +1306,7 @@ int fop_of(int dop) {
         EK_FOPS0(X)
         X(TAN_F32) X(COT_F32) X(ASIN_F32) X(ACOS_F32) X(ATAN_F32) X(ATAN2_F32) X(ATAN2R_F32)
         X(SINH_F32) X(COSH_F32) X(TANH_F32) X(ASINH_F32) X(ACOSH_F32) X(ATANH_F32) X(CBRT_F32)
+        X(ERF_F32) X(ERFC_F32) X(ERFINV_F32) X(LGAMMA_F32) X(TGAMMA_F32)
 #undef X
         case DOP_LOAD_32: return FOP_LOAD;
         default: return -1;
@@ -1803,7 +1811,7 @@ void write_program_json(std::ostream &os, const EkContext &ctx, const std::vecto
             EK_FOPS2(X)
 #undef X
 #define X(n) #n,
-            EK_FOPS1(X) EK_FOPS0(X) EK_FOPS16(X) EK_FOPST(X) EK_FOPSH(X)
+            EK_FOPS1(X) EK_FOPS0(X) EK_FOPS16(X) EK_FOPST(X) EK_FOPSH(X) EK_FOPSS(X)
 #undef X
         };
         for (int k = 0; k < FOP__COUNT; ++k) os << (k ? "," : "") << "\"" << fnames[k] << "\"";
@@ -1905,7 +1913,7 @@ bool launch_sweep(EkContext &ctx, const Sweep &s) {
     if (cfg.fast) {
         ek_cuda_check(ek_launch_sweep_fast(args, grid, cfg.T, cfg.smem, ctx.stream));
     } else {
-        bool trig = false;          /* the general kernel's instantiation with the trigonometric and hyperbolic operations */
+        bool trig = false;          /* the general kernel's instantiation with the trigonometric, hyperbolic and special operations */
         for (const EkInstr &in : a.body) trig |= ek_dop_ext(in.op);
         ek_cuda_check(ek_launch_sweep(cfg.V, inline_prog, trig, args, grid, cfg.T, cfg.smem, ctx.stream));
     }

@@ -134,11 +134,12 @@ struct EkInstr {
     /* init/fini helpers for privatised scatter_add bins and staged gather tables \
        (imm = descriptor index in the uniform pool; SMEM_ZERO: dst = 1 for float bins, which start at -0.0) */ \
     X(SMEM_ZERO) X(SMEM_LOAD_TABLE) X(SMEM_FLUSH_ADD_F32) X(SMEM_FLUSH_ADD_I32) \
-    /* f32 trigonometric and hyperbolic functions of array_math.h (ek_math.cuh), numbered last so that the operations \
-       above keep their numbers (ek_sweep_kernel<V, INLINE, false> carries none of them: ek_dop_ext); ATAN2: R = y, \
-       B = x, ATAN2R: R = x, B = y */ \
+    /* f32 trigonometric and hyperbolic functions of array_math.h and special functions of special.h (ek_math.cuh), \
+       numbered last so that the operations above keep their numbers (ek_sweep_kernel<V, INLINE, false> carries none \
+       of them: ek_dop_ext); ATAN2: R = y, B = x, ATAN2R: R = x, B = y */ \
     X(TAN_F32) X(COT_F32) X(ASIN_F32) X(ACOS_F32) X(ATAN_F32) X(ATAN2_F32) X(ATAN2R_F32) \
-    X(SINH_F32) X(COSH_F32) X(TANH_F32) X(ASINH_F32) X(ACOSH_F32) X(ATANH_F32) X(CBRT_F32)
+    X(SINH_F32) X(COSH_F32) X(TANH_F32) X(ASINH_F32) X(ACOSH_F32) X(ATANH_F32) X(CBRT_F32) \
+    X(ERF_F32) X(ERFC_F32) X(ERFINV_F32) X(LGAMMA_F32) X(TGAMMA_F32)
 
 enum EkDop : uint16_t {
 #define X(n) DOP_##n,
@@ -148,8 +149,8 @@ enum EkDop : uint16_t {
 };
 
 /* the operations that only the extension instantiations of the sweep kernels carry (ek_sweep_kernel<V, INLINE, true>;
-   lowered, ek_fast_kernel<T, EK_FX_TRIG / EK_FX_HYP>): tan ... cbrt, numbered after every other operation.  The imm field of these
-   instructions is free, and a body that contains one runs on those instantiations. */
+   lowered, ek_fast_kernel<T, EK_FX_TRIG / EK_FX_HYP / EK_FX_SPEC>): tan ... tgamma, numbered after every other
+   operation.  The imm field of these instructions is free, and a body that contains one runs on those instantiations. */
 static inline bool ek_dop_ext(uint32_t op) { return op >= DOP_TAN_F32 && op < DOP__COUNT; }
 
 /* ---- lowered instruction format of the 32-bit fast kernel (ek_sweep_fast.cu) ----
@@ -206,13 +207,16 @@ static inline bool ek_dop_ext(uint32_t op) { return op >= DOP_TAN_F32 && op < DO
                     X(ATAN2_F32) X(ATAN2_F32_U) X(ATAN2R_F32) X(ATAN2R_F32_U)
 /* sinh, cosh, tanh, asinh, acosh, atanh and cbrt, in the bodies that the hyp instantiations run (numbered last) */
 #define EK_FOPSH(X) X(SINH_F32) X(COSH_F32) X(TANH_F32) X(ASINH_F32) X(ACOSH_F32) X(ATANH_F32) X(CBRT_F32)
+/* erf, erfc, erfinv, lgamma and tgamma, in the bodies that the special-function instantiations run (numbered last) */
+#define EK_FOPSS(X) X(ERF_F32) X(ERFC_F32) X(ERFINV_F32) X(LGAMMA_F32) X(TGAMMA_F32)
 
 /* feature bits of the ek_fast_kernel instantiations: the launcher runs the smallest one whose operations cover the
    lowered body */
 #define EK_FX_F16  1u     /* FOP_LD_F16, FOP_ST_F16 */
 #define EK_FX_TRIG 2u     /* EK_FOPST */
 #define EK_FX_HYP  4u     /* EK_FOPSH */
-#define EK_FX_ALL  (EK_FX_F16 | EK_FX_TRIG | EK_FX_HYP)
+#define EK_FX_SPEC 8u     /* EK_FOPSS */
+#define EK_FX_ALL  (EK_FX_F16 | EK_FX_TRIG | EK_FX_HYP | EK_FX_SPEC)
 
 enum EkFop : uint16_t {
     FOP_NOP,
@@ -225,6 +229,7 @@ enum EkFop : uint16_t {
     EK_FOPS16(X)
     EK_FOPST(X)
     EK_FOPSH(X)
+    EK_FOPSS(X)
 #undef X
     FOP__COUNT
 };
@@ -235,7 +240,8 @@ static inline uint32_t ek_fast_ext(const EkInstr *body, uint32_t n) {
     for (uint32_t pc = 0; pc < n; ++pc) {
         const uint32_t op = body[pc].op;
         if (op == FOP_LD_F16 || op == FOP_ST_F16) ext |= EK_FX_F16;
-        else if (op >= FOP_SINH_F32 && op < FOP__COUNT) ext |= EK_FX_HYP;
+        else if (op >= FOP_ERF_F32 && op < FOP__COUNT) ext |= EK_FX_SPEC;
+        else if (op >= FOP_SINH_F32 && op <= FOP_CBRT_F32) ext |= EK_FX_HYP;
         else if (op >= FOP_TAN_F32) ext |= EK_FX_TRIG;
     }
     return ext;

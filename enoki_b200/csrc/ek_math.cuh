@@ -316,6 +316,88 @@ __device__ __forceinline__ float cbrt_f32(float x) {
     return fabsf(x) < __int_as_float(0x7f800000) ? r : x;
 }
 
+/* ---------------- erf, erfc, erfinv, lgamma, tgamma ----------------
+   The single precision branches of special.h, restated the same way: the operation sequence that the generic body
+   records on this backend, with this backend's exp_f32 / log_f32 / sin_f32, the correctly rounded rcp and division,
+   rintf for round (ROUND_F32), negation as a sign flip (NEG_F32) and the coefficients rounded to float as Scalar(c)
+   rounds them.  On a CUDA array both sides of every branch are recorded and selected; evaluating only the selected
+   side gives the same bits. */
+
+/* array_math.h:65-72 */
+__device__ __forceinline__ float poly7(float x, float c0, float c1, float c2, float c3, float c4, float c5, float c6,
+                                       float c7) {
+    float x2 = fmul(x, x), x4 = fmul(x2, x2);
+    return ffma(x4, ffma(x2, ffma(x, c7, c6), ffma(x, c5, c4)), ffma(x2, ffma(x, c3, c2), ffma(x, c1, c0)));
+}
+__device__ __forceinline__ float fneg(float x) { return fbits(ubits(x) ^ 0x80000000u); }
+
+/* special.h:56-129 erfc<T, false>, single precision branch (the body without its |x| < 1 recursion into erf) */
+__device__ __forceinline__ float erfc_core_f32(float x) {
+    float xa = fabsf(x), q = __frcp_rn(xa), y = fmul(q, q);
+    float p_small = poly8(y, (float) 5.638259427386472e-1, (float) -2.741127028184656e-1, (float) 3.404879937665872e-1,
+                             (float) -4.944515323274145e-1, (float) 6.210004621745983e-1, (float) -5.824733027278666e-1,
+                             (float) 3.687424674597105e-1, (float) -1.387039388740657e-1, (float) 2.326819970068386e-2);
+    float p_large = poly7(y, (float) 5.641895067754075e-1, (float) -2.820767439740514e-1, (float) 4.218463358204948e-1,
+                             (float) -1.015265279202700e+0, (float) 2.921019019210786e+0, (float) -7.495518717768503e+0,
+                             (float) 1.297719955372516e+1, (float) -1.047766399936249e+1);
+    float r = fmul(fmul(exp_f32(fmul(fneg(x), x)), q), xa > 2.f ? p_large : p_small);
+    return x < 0.f ? fsub(2.f, r) : r;                                            /* r[x < 0] = 2 - r */
+}
+/* special.h:131-164 erf<T, false>, single precision branch (the body without its |x| > 1 recursion into erfc) */
+__device__ __forceinline__ float erf_core_f32(float x) {
+    float r = poly6(fmul(x, x), (float) 1.128379165726710e+0, (float) -3.761262582423300e-1,
+                                (float) 1.128358514861418e-1, (float) -2.685381193529856e-2,
+                                (float) 5.188327685732524e-3, (float) -8.010193625184903e-4,
+                                (float) 7.853861353153693e-5);
+    return fmul(r, x);
+}
+/* special.h:131-164 erf: r[|x| > 1] = 1 - erfc<T, false>(x) */
+__device__ __forceinline__ float erf_f32(float x) {
+    return fabsf(x) > 1.f ? fsub(1.f, erfc_core_f32(x)) : erf_core_f32(x);
+}
+/* special.h:56-129 erfc: r[|x| < 1] = 1 - erf<T, false>(x).  At |x| == 1 erf takes its polynomial and erfc its own
+   formula. */
+__device__ __forceinline__ float erfc_f32(float x) {
+    return fabsf(x) < 1.f ? fsub(1.f, erf_core_f32(x)) : erfc_core_f32(x);
+}
+
+/* special.h:222-246 erfinv */
+__device__ __forceinline__ float erfinv_f32(float x) {
+    float w = fneg(log_f32(fmul(fadd(1.f, x), fsub(1.f, x))));
+    float w1 = fsub(w, 2.5f), w2 = fsub(__fsqrt_rn(w), 3.f);
+    float p1 = poly8(w1, (float) 1.50140941, (float) 0.246640727, (float) -0.00417768164, (float) -0.00125372503,
+                         (float) 0.00021858087, (float) -4.39150654e-06, (float) -3.5233877e-06, (float) 3.43273939e-07,
+                         (float) 2.81022636e-08);
+    float p2 = poly8(w2, (float) 2.83297682, (float) 1.00167406, (float) 0.00943887047, (float) -0.0076224613,
+                         (float) 0.00573950773, (float) -0.00367342844, (float) 0.00134934322, (float) 0.000100950558,
+                         (float) -0.000200214257);
+    return fmul(w < 5.f ? p1 : p2, x);
+}
+
+/* special.h:275-309 lgamma (Lanczos, g = 5, n = 6).  The sum starts from a recorded literal 0, so a -0 quotient becomes
+   +0; b = (x + 5) + 0.5 rounds twice. */
+__device__ __forceinline__ float lgamma_f32(float x_) {
+    const float pi = (float) 3.14159265358979323846;
+    bool reflect = x_ < 0.5f;
+    float x = reflect ? fneg(x_) : fsub(x_, 1.f);
+    float sum = fadd(__fdiv_rn((float) -0.5395239384953e-5, fadd(x, 6.f)), 0.f);
+    sum = fadd(sum, __fdiv_rn((float) 0.1208650973866179e-2, fadd(x, 5.f)));
+    sum = fadd(sum, __fdiv_rn((float) -1.231739572450155, fadd(x, 4.f)));
+    sum = fadd(sum, __fdiv_rn((float) 24.01409824083091, fadd(x, 3.f)));
+    sum = fadd(sum, __fdiv_rn((float) -86.50532032941677, fadd(x, 2.f)));
+    sum = fadd(sum, __fdiv_rn((float) 76.18009172947146, fadd(x, 1.f)));
+    sum = fadd(sum, (float) 1.000000000190015);
+    float b = fadd(fadd(x, 5.f), 0.5f);
+    float result = fadd(fsub(fadd((float) 0.91893853320467274178, log_f32(sum)), b), fmul(log_f32(b), fadd(x, 0.5f)));
+    if (reflect) {
+        result = fsub(log_f32(fabsf(__fdiv_rn(pi, sin_f32(fmul(pi, x_))))), result);
+        if (x_ == rintf(x_)) result = __int_as_float(0x7f800000);
+    }
+    return result;
+}
+/* special.h:312 tgamma = exp(lgamma(x)) */
+__device__ __forceinline__ float tgamma_f32(float x) { return exp_f32(lgamma_f32(x)); }
+
 /* ---------------- two elements at a time ----------------
    The sweep kernels evaluate exp / sin / cos on pairs of elements: the two independent dependency chains give
    ptxas instruction-level parallelism to interleave.  sm_90 has no packed fp32 arithmetic, so every pair

@@ -52,7 +52,8 @@ const char *ek_op_name(ek_op op) {
         "popc", "clz", "ctz", "add", "sub", "mul", "mulhi", "div", "mod", "min", "max", "shl", "shr",
         "and", "or", "xor", "gt", "ge", "lt", "le", "eq", "ne", "mul_nz", "fma", "select", "fma_nz",
         "gather", "scatter", "scatter_add", "hsum", "hprod", "hmax", "hmin", "all", "any", "count", "printf",
-        "tan", "cot", "asin", "acos", "atan", "atan2", "sinh", "cosh", "tanh", "asinh", "acosh", "atanh", "cbrt" };
+        "tan", "cot", "asin", "acos", "atan", "atan2", "sinh", "cosh", "tanh", "asinh", "acosh", "atanh", "cbrt",
+        "erf", "erfc", "erfinv", "lgamma", "tgamma" };
     return (unsigned) op < EK_OP__COUNT ? names[op] : "?";
 }
 

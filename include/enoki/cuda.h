@@ -238,6 +238,13 @@ struct CUDAArray : ArrayBase<value_t<Value>, CUDAArray<Value>> {
     /// (DiffArray's sinh_ / cosh_ call it)
     template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0>
     std::pair<CUDAArray, CUDAArray> sincosh_() const { return { sinh_(), cosh_() }; }
+    /// erf/erfc/erfinv/lgamma/tgamma: the same for the special functions (special.h:56-164,222-246,275-312).  special.h
+    /// calls no members, so the free overloads of CUDAArray<float> below are the entry points that use these.
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray erf_() const { return un_(EK_OP_ERF); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray erfc_() const { return un_(EK_OP_ERFC); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray erfinv_() const { return un_(EK_OP_ERFINV); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray lgamma_() const { return un_(EK_OP_LGAMMA); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray tgamma_() const { return un_(EK_OP_TGAMMA); }
     CUDAArray floor_() const { return un_(EK_OP_FLOOR); }
     CUDAArray ceil_() const { return un_(EK_OP_CEIL); }
     CUDAArray round_() const { return un_(EK_OP_ROUND); }
@@ -471,6 +478,16 @@ protected:
     mutable std::vector<std::pair<Value, CUDAArray<uint32_t>>> *m_cached_partition = nullptr;
 };
 static_assert(sizeof(CUDAArray<float>) == 16, "CUDAArray<T> must keep the reference's 16-byte layout");
+
+/// special.h's erf, erfc, erfinv, lgamma and tgamma are free templates.  These non-template overloads are exact matches
+/// for a CUDAArray<float>, so they win over the templates, and argument-dependent lookup finds them whichever of the two
+/// headers comes first.  erf<FloatC>(x) with explicit template arguments still records special.h's body op by op, and
+/// DiffArray, nested arrays and CUDAArray<double> keep the templates.
+inline CUDAArray<float> erf(const CUDAArray<float> &x) { return x.erf_(); }
+inline CUDAArray<float> erfc(const CUDAArray<float> &x) { return x.erfc_(); }
+inline CUDAArray<float> erfinv(const CUDAArray<float> &x) { return x.erfinv_(); }
+inline CUDAArray<float> lgamma(const CUDAArray<float> &x) { return x.lgamma_(); }
+inline CUDAArray<float> tgamma(const CUDAArray<float> &x) { return x.tgamma_(); }
 
 template <typename T, enable_if_t<!is_diff_array_v<T> && is_cuda_array_v<T>> = 0>
 ENOKI_INLINE void set_label(const T &a, const char *label) {

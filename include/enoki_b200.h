@@ -132,6 +132,11 @@ typedef enum ek_op {
     EK_OP_ACOSH,       /* array_math.h:1239-1293 */
     EK_OP_ATANH,       /* array_math.h:1295-1348 */
     EK_OP_CBRT,        /* array_math.h:900-954  frexp :682-709, ldexp :677-680              */
+    EK_OP_ERF,         /* special.h:131-164 */
+    EK_OP_ERFC,        /* special.h:56-129 */
+    EK_OP_ERFINV,      /* special.h:222-246 */
+    EK_OP_LGAMMA,      /* special.h:275-309 */
+    EK_OP_TGAMMA,      /* special.h:312     exp(lgamma(x))                                  */
     EK_OP__COUNT
 } ek_op;
 
