@@ -28,6 +28,11 @@ _OPS = ["INVALID", "LITERAL", "INDEX", "MOV", "CVT", "BITCAST", "NEG", "ABS", "S
 # operations (EK_FX_SPEC)
 _OPS_SPECIAL = ["ERF", "ERFC", "ERFINV", "LGAMMA", "TGAMMA"]
 OP = {n: i for i, n in enumerate(_OPS + _OPS_SPECIAL)}
+# the remaining Float32 functions of array_math.h and special.h, numbered after EK_OP_TGAMMA (their sweep operations:
+# EK_FX_MATH); a table of their own, so that OP keeps the opcodes it held before they existed
+_OPS_MATH = ["POW", "FREXP_M", "FREXP_E", "HYPOT", "DAWSON", "ERFI"]
+OP_MATH = {n: len(OP) + i for i, n in enumerate(_OPS_MATH)}
+_OPCODE = {**OP, **OP_MATH}
 
 _NP = {EK_INT8: np.int8, EK_UINT8: np.uint8, EK_INT16: np.int16, EK_UINT16: np.uint16,
        EK_INT32: np.int32, EK_UINT32: np.uint32, EK_INT64: np.int64, EK_UINT64: np.uint64,
@@ -49,7 +54,7 @@ def _check(handle_or_rc, ok):
 
 
 def _append(t, op, a=0, b=0, c=0, imm=0):
-    h = lib().ek_trace_append(t, OP[op], a, b, c, imm)
+    h = lib().ek_trace_append(t, _OPCODE[op], a, b, c, imm)
     return _check(h, h != 0)
 
 
@@ -264,6 +269,28 @@ def atan2(y, x):
     cls = next(type(v) for v in (y, x) if isinstance(v, CUDAArray))
     y, x = (v if isinstance(v, CUDAArray) else cls(v) for v in (y, x))
     return y._bin("ATAN2", x)
+
+
+# Float32 only: one node each, bit for bit the single precision bodies of array_math.h and special.h (DESIGN.md 4)
+dawson, erfi = (_unary(o) for o in ("DAWSON", "ERFI"))
+
+
+def _binary(op, doc):
+    def f(x, y):
+        cls = next(type(v) for v in (x, y) if isinstance(v, CUDAArray))
+        x, y = (v if isinstance(v, CUDAArray) else cls(v) for v in (x, y))
+        return x._bin(op, y)
+    f.__name__, f.__doc__ = op.lower(), doc
+    return f
+
+
+pow_ = _binary("POW", "pow(x, y) = exp(log(x) * y) (array_math.h:956-958); either operand may be a Python number")
+hypot = _binary("HYPOT", "hypot(a, b) (array_math.h:1362-1379); either operand may be a Python number")
+
+
+def frexp(x):
+    """(mantissa, exponent) of array_math.h:682-709, both Float32"""
+    return x._un("FREXP_M"), x._un("FREXP_E")
 
 
 def sincos(x):

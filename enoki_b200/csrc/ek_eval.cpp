@@ -160,6 +160,12 @@ int pick_op(ek_op op, ek_type vt, ek_type at /* operand type */) {
         case EK_OP_ERFINV: return SEL(DOP_ERFINV_F32, -1, -1, -1, -1, -1);
         case EK_OP_LGAMMA: return SEL(DOP_LGAMMA_F32, -1, -1, -1, -1, -1);
         case EK_OP_TGAMMA: return SEL(DOP_TGAMMA_F32, -1, -1, -1, -1, -1);
+        case EK_OP_POW:     return SEL(DOP_POW_F32, -1, -1, -1, -1, -1);
+        case EK_OP_FREXP_M: return SEL(DOP_FREXP_M_F32, -1, -1, -1, -1, -1);
+        case EK_OP_FREXP_E: return SEL(DOP_FREXP_E_F32, -1, -1, -1, -1, -1);
+        case EK_OP_HYPOT:   return SEL(DOP_HYPOT_F32, -1, -1, -1, -1, -1);
+        case EK_OP_DAWSON:  return SEL(DOP_DAWSON_F32, -1, -1, -1, -1, -1);
+        case EK_OP_ERFI:    return SEL(DOP_ERFI_F32, -1, -1, -1, -1, -1);
         case EK_OP_FLOOR: return SEL(DOP_FLOOR_F32, DOP_FLOOR_F64, DOP_LOAD_32, DOP_LOAD_32, DOP_LOAD_64, DOP_LOAD_64);
         case EK_OP_CEIL:  return SEL(DOP_CEIL_F32, DOP_CEIL_F64, DOP_LOAD_32, DOP_LOAD_32, DOP_LOAD_64, DOP_LOAD_64);
         case EK_OP_ROUND: return SEL(DOP_ROUND_F32, DOP_ROUND_F64, DOP_LOAD_32, DOP_LOAD_32, DOP_LOAD_64, DOP_LOAD_64);
@@ -921,7 +927,8 @@ struct Assembler {
                             case EK_OP_GE: eop = EK_OP_LE; break;
                             case EK_OP_LT: eop = EK_OP_GT; break;
                             case EK_OP_LE: eop = EK_OP_GE; break;
-                            case EK_OP_SUB: case EK_OP_DIV: case EK_OP_MOD: case EK_OP_SHL: case EK_OP_SHR: case EK_OP_ATAN2: reversed = true; break;
+                            case EK_OP_SUB: case EK_OP_DIV: case EK_OP_MOD: case EK_OP_SHL: case EK_OP_SHR: case EK_OP_ATAN2:
+                            case EK_OP_POW: case EK_OP_HYPOT: reversed = true; break;
                             case EK_OP_MIN: case EK_OP_MAX: reversed = ek_is_float(t); break;
                             default: break;       /* commutative */
                         }
@@ -1040,6 +1047,7 @@ struct Assembler {
     static int reversed_op(int dop) {
         switch (dop) {
             case DOP_SUB_F32: return DOP_SUBR_F32; case DOP_DIV_F32: return DOP_DIVR_F32; case DOP_ATAN2_F32: return DOP_ATAN2R_F32;
+            case DOP_POW_F32: return DOP_POWR_F32; case DOP_HYPOT_F32: return DOP_HYPOTR_F32;
             case DOP_MIN_F32: return DOP_MINR_F32; case DOP_MAX_F32: return DOP_MAXR_F32;
             case DOP_SUB_F64: return DOP_SUBR_F64; case DOP_DIV_F64: return DOP_DIVR_F64;
             case DOP_MIN_F64: return DOP_MINR_F64; case DOP_MAX_F64: return DOP_MAXR_F64;
@@ -1088,6 +1096,11 @@ struct Assembler {
                              case DOP_CBRT_F32: return 16.0;
                              case DOP_ERF_F32: case DOP_ERFC_F32: case DOP_ERFINV_F32: return 14.0;
                              case DOP_LGAMMA_F32: case DOP_TGAMMA_F32: return 20.0;
+                             case DOP_POW_F32: case DOP_POWR_F32: return 16.0;
+                             case DOP_FREXP_M_F32: case DOP_FREXP_E_F32: return 2.0;
+                             case DOP_HYPOT_F32: case DOP_HYPOTR_F32: return 8.0;
+                             case DOP_DAWSON_F32: return 6.0;
+                             case DOP_ERFI_F32: return 14.0;
                              case DOP_SQRT_F32: case DOP_DIV_F32: case DOP_RCP_F32: case DOP_RSQRT_F32: return 3.0; default: return 1.0; } };
         double total_w = 0; for (const EkInstr &in : out.body) total_w += weight(in);
         double acc_w = 0;
@@ -1307,6 +1320,7 @@ int fop_of(int dop) {
         X(TAN_F32) X(COT_F32) X(ASIN_F32) X(ACOS_F32) X(ATAN_F32) X(ATAN2_F32) X(ATAN2R_F32)
         X(SINH_F32) X(COSH_F32) X(TANH_F32) X(ASINH_F32) X(ACOSH_F32) X(ATANH_F32) X(CBRT_F32)
         X(ERF_F32) X(ERFC_F32) X(ERFINV_F32) X(LGAMMA_F32) X(TGAMMA_F32)
+        X(POW_F32) X(POWR_F32) X(FREXP_M_F32) X(FREXP_E_F32) X(HYPOT_F32) X(HYPOTR_F32) X(DAWSON_F32) X(ERFI_F32)
 #undef X
         case DOP_LOAD_32: return FOP_LOAD;
         default: return -1;
@@ -1318,6 +1332,7 @@ bool fop_has_u_twin(int fop) {
         EK_FOPS2(X)
 #undef X
         case FOP_ATAN2_F32: case FOP_ATAN2R_F32:
+        case FOP_POW_F32: case FOP_POWR_F32: case FOP_HYPOT_F32: case FOP_HYPOTR_F32:
             return true;
         default: return false;
     }
@@ -1426,7 +1441,7 @@ bool lower_fast(const std::vector<EkInstr> &in, const Assembled &a, const Config
                 dst = i.dst;
                 break;
             default:
-                if (hb && ub && !hc && fop_has_u_twin(fop)) fop += 1;          /* X_U = X + 1 */
+                if (hb && ub && !hc && fop_has_u_twin(fop)) fop += 1;          /* X_U (X_UB) = X + 1 */
                 else {
                     if (hb) fl |= ub ? FF_BU : FF_B;
                     if (hc) fl |= uc ? FF_CU : FF_C;
@@ -1811,7 +1826,7 @@ void write_program_json(std::ostream &os, const EkContext &ctx, const std::vecto
             EK_FOPS2(X)
 #undef X
 #define X(n) #n,
-            EK_FOPS1(X) EK_FOPS0(X) EK_FOPS16(X) EK_FOPST(X) EK_FOPSH(X) EK_FOPSS(X)
+            EK_FOPS1(X) EK_FOPS0(X) EK_FOPS16(X) EK_FOPST(X) EK_FOPSH(X) EK_FOPSS(X) EK_FOPSM(X)
 #undef X
         };
         for (int k = 0; k < FOP__COUNT; ++k) os << (k ? "," : "") << "\"" << fnames[k] << "\"";
@@ -1913,7 +1928,7 @@ bool launch_sweep(EkContext &ctx, const Sweep &s) {
     if (cfg.fast) {
         ek_cuda_check(ek_launch_sweep_fast(args, grid, cfg.T, cfg.smem, ctx.stream));
     } else {
-        bool trig = false;          /* the general kernel's instantiation with the trigonometric, hyperbolic and special operations */
+        bool trig = false;          /* the general kernel's instantiation with the trigonometric, hyperbolic, special and other math operations */
         for (const EkInstr &in : a.body) trig |= ek_dop_ext(in.op);
         ek_cuda_check(ek_launch_sweep(cfg.V, inline_prog, trig, args, grid, cfg.T, cfg.smem, ctx.stream));
     }

@@ -102,7 +102,7 @@ void ek_cuda_check_impl(cudaError_t err, const char *file, int line);
 #define ek_cuda_check(x) ek_cuda_check_impl((x), __FILE__, __LINE__)
 
 /* kernels (defined in .cu files) */
-/* trig: the body contains an operation of the extension instantiations (ek_isa.h ek_dop_ext: tan ... tgamma) */
+/* trig: the body contains an operation of the extension instantiations (ek_isa.h ek_dop_ext: tan ... erfi) */
 cudaError_t ek_launch_sweep(int V, bool inline_prog, bool trig, const EkSweepArgs &args, unsigned grid, unsigned block,
                             size_t smem_bytes, cudaStream_t stream);
 /* 32-bit fast kernel (ek_sweep_fast.cu): args.prog_inline holds the lowered program; block = 128 or 256 */
@@ -130,12 +130,15 @@ static inline bool ek_is_signed(ek_type t) {
 static inline bool ek_is_64(ek_type t) { return ek_type_size(t) == 8; }
 const char *ek_type_name(ek_type t);
 const char *ek_op_name(ek_op op);
-/* element-wise operations of one and of two operands (the trigonometric, hyperbolic and special ones come after
-   EK_OP_PRINTF) */
+/* element-wise operations of one and of two operands (the trigonometric, hyperbolic, special and remaining Float32
+   math ones come after EK_OP_PRINTF) */
 static inline bool ek_op_unary(ek_op op) {
-    return (op >= EK_OP_MOV && op <= EK_OP_CTZ) || (op >= EK_OP_TAN && op <= EK_OP_ATAN) || (op >= EK_OP_SINH && op <= EK_OP_TGAMMA);
+    return (op >= EK_OP_MOV && op <= EK_OP_CTZ) || (op >= EK_OP_TAN && op <= EK_OP_ATAN) || (op >= EK_OP_SINH && op <= EK_OP_TGAMMA) ||
+           op == EK_OP_FREXP_M || op == EK_OP_FREXP_E || op == EK_OP_DAWSON || op == EK_OP_ERFI;
 }
-static inline bool ek_op_binary(ek_op op) { return (op >= EK_OP_ADD && op <= EK_OP_MUL_NZ) || op == EK_OP_ATAN2; }
+static inline bool ek_op_binary(ek_op op) {
+    return (op >= EK_OP_ADD && op <= EK_OP_MUL_NZ) || op == EK_OP_ATAN2 || op == EK_OP_POW || op == EK_OP_HYPOT;
+}
 
 /* cuda_printf formats (ek_printf.cpp).  A parsed format is a list of segments: literal text (conv == 0, "%%" already
    reduced to "%") or one conversion, `text` being its spec as written ("%-08.3lx") and `arg` the argument it takes. */

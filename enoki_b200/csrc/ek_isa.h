@@ -139,7 +139,9 @@ struct EkInstr {
        of them: ek_dop_ext); ATAN2: R = y, B = x, ATAN2R: R = x, B = y */ \
     X(TAN_F32) X(COT_F32) X(ASIN_F32) X(ACOS_F32) X(ATAN_F32) X(ATAN2_F32) X(ATAN2R_F32) \
     X(SINH_F32) X(COSH_F32) X(TANH_F32) X(ASINH_F32) X(ACOSH_F32) X(ATANH_F32) X(CBRT_F32) \
-    X(ERF_F32) X(ERFC_F32) X(ERFINV_F32) X(LGAMMA_F32) X(TGAMMA_F32)
+    X(ERF_F32) X(ERFC_F32) X(ERFINV_F32) X(LGAMMA_F32) X(TGAMMA_F32) \
+    /* further f32 functions of array_math.h and special.h; POW / HYPOT: R = x, B = y, POWR / HYPOTR: R = y, B = x */ \
+    X(POW_F32) X(POWR_F32) X(FREXP_M_F32) X(FREXP_E_F32) X(HYPOT_F32) X(HYPOTR_F32) X(DAWSON_F32) X(ERFI_F32)
 
 enum EkDop : uint16_t {
 #define X(n) DOP_##n,
@@ -149,7 +151,7 @@ enum EkDop : uint16_t {
 };
 
 /* the operations that only the extension instantiations of the sweep kernels carry (ek_sweep_kernel<V, INLINE, true>;
-   lowered, ek_fast_kernel<T, EK_FX_TRIG / EK_FX_HYP / EK_FX_SPEC>): tan ... tgamma, numbered after every other
+   lowered, ek_fast_kernel<T, EK_FX_TRIG / EK_FX_HYP / EK_FX_SPEC / EK_FX_MATH>): tan ... erfi, numbered after every other
    operation.  The imm field of these instructions is free, and a body that contains one runs on those instantiations. */
 static inline bool ek_dop_ext(uint32_t op) { return op >= DOP_TAN_F32 && op < DOP__COUNT; }
 
@@ -209,6 +211,11 @@ static inline bool ek_dop_ext(uint32_t op) { return op >= DOP_TAN_F32 && op < DO
 #define EK_FOPSH(X) X(SINH_F32) X(COSH_F32) X(TANH_F32) X(ASINH_F32) X(ACOSH_F32) X(ATANH_F32) X(CBRT_F32)
 /* erf, erfc, erfinv, lgamma and tgamma, in the bodies that the special-function instantiations run (numbered last) */
 #define EK_FOPSS(X) X(ERF_F32) X(ERFC_F32) X(ERFINV_F32) X(LGAMMA_F32) X(TGAMMA_F32)
+/* pow, frexp, hypot, dawson and erfi, in the bodies that the EK_FX_MATH instantiations run (numbered last).
+   The binary ones: the accumulator is x (R forms: y); _UB = X + 1: the other operand is uniform-pool word b (as
+   FMA_F32_UB) */
+#define EK_FOPSM(X) X(POW_F32) X(POW_F32_UB) X(POWR_F32) X(POWR_F32_UB) X(FREXP_M_F32) X(FREXP_E_F32) \
+                    X(HYPOT_F32) X(HYPOT_F32_UB) X(HYPOTR_F32) X(HYPOTR_F32_UB) X(DAWSON_F32) X(ERFI_F32)
 
 /* feature bits of the ek_fast_kernel instantiations: the launcher runs the smallest one whose operations cover the
    lowered body */
@@ -216,7 +223,8 @@ static inline bool ek_dop_ext(uint32_t op) { return op >= DOP_TAN_F32 && op < DO
 #define EK_FX_TRIG 2u     /* EK_FOPST */
 #define EK_FX_HYP  4u     /* EK_FOPSH */
 #define EK_FX_SPEC 8u     /* EK_FOPSS */
-#define EK_FX_ALL  (EK_FX_F16 | EK_FX_TRIG | EK_FX_HYP | EK_FX_SPEC)
+#define EK_FX_MATH 16u    /* EK_FOPSM */
+#define EK_FX_ALL  (EK_FX_F16 | EK_FX_TRIG | EK_FX_HYP | EK_FX_SPEC | EK_FX_MATH)
 
 enum EkFop : uint16_t {
     FOP_NOP,
@@ -230,6 +238,7 @@ enum EkFop : uint16_t {
     EK_FOPST(X)
     EK_FOPSH(X)
     EK_FOPSS(X)
+    EK_FOPSM(X)
 #undef X
     FOP__COUNT
 };
@@ -240,7 +249,8 @@ static inline uint32_t ek_fast_ext(const EkInstr *body, uint32_t n) {
     for (uint32_t pc = 0; pc < n; ++pc) {
         const uint32_t op = body[pc].op;
         if (op == FOP_LD_F16 || op == FOP_ST_F16) ext |= EK_FX_F16;
-        else if (op >= FOP_ERF_F32 && op < FOP__COUNT) ext |= EK_FX_SPEC;
+        else if (op >= FOP_POW_F32 && op < FOP__COUNT) ext |= EK_FX_MATH;
+        else if (op >= FOP_ERF_F32 && op <= FOP_TGAMMA_F32) ext |= EK_FX_SPEC;
         else if (op >= FOP_SINH_F32 && op <= FOP_CBRT_F32) ext |= EK_FX_HYP;
         else if (op >= FOP_TAN_F32) ext |= EK_FX_TRIG;
     }

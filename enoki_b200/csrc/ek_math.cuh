@@ -398,6 +398,52 @@ __device__ __forceinline__ float lgamma_f32(float x_) {
 /* special.h:312 tgamma = exp(lgamma(x)) */
 __device__ __forceinline__ float tgamma_f32(float x) { return exp_f32(lgamma_f32(x)); }
 
+/* ---------------- pow, frexp, hypot, dawson, erfi ----------------
+   Further single precision bodies of array_math.h and special.h, restated the same way: this backend's exp_f32 /
+   log_f32, the correctly rounded division and sqrt, min / max with the x86 operand rule, and the coefficients rounded to
+   float as Scalar(c) rounds them. */
+
+/* array_math.h:956-958 pow = exp(log(x) * y): pow(0, 0) = exp(-inf * 0) is NaN, as is the power of a negative base */
+__device__ __forceinline__ float pow_f32(float x, float y) { return exp_f32(fmul(log_f32(x), y)); }
+
+/* array_math.h:682-709 frexp: (mantissa | 0.5, biased exponent - 0x7f) for every number whose exponent field is not all
+   ones except +-0, denormals included (their mantissa keeps its leading zeros, their exponent is -127); (x, 0) for
+   +-0, +-inf and NaN */
+__device__ __forceinline__ bool frexp_normal(float x) { return x != 0.f && (ubits(x) & 0x7f800000u) != 0x7f800000u; }
+__device__ __forceinline__ float frexp_m_f32(float x) {
+    return frexp_normal(x) ? fbits((ubits(x) & ~0x7f800000u) | 0x3f000000u) : x;
+}
+__device__ __forceinline__ float frexp_e_f32(float x) {
+    return __int2float_rn(frexp_normal(x) ? (int32_t) ((ubits(x) & 0x7f800000u) >> 23) - 0x7f : 0);
+}
+
+/* array_math.h:1362-1379 hypot: max * sqrt(1 + (min / max)^2) where both operands and the ratio are finite, |a| + |b|
+   elsewhere */
+__device__ __forceinline__ float hypot_f32(float a, float b) {
+    const float inf = __int_as_float(0x7f800000);
+    float abs_a = fabsf(a), abs_b = fabsf(b);
+    float maxval = max_x86(abs_a, abs_b), minval = min_x86(abs_a, abs_b), ratio = __fdiv_rn(minval, maxval);
+    return abs_a < inf && abs_b < inf && ratio < inf ? fmul(maxval, __fsqrt_rn(fadd(1.f, fmul(ratio, ratio))))
+                                                     : fadd(abs_a, abs_b);
+}
+
+/* special.h:249-265 dawson = num(x^2) / denom(x^2) * x */
+__device__ __forceinline__ float dawson_f32(float x) {
+    float x2 = fmul(x, x);
+    float num = poly6(x2, (float) 1.00000080272429, (float) 9.18170212243285e-2, (float) 4.25835373536124e-2,
+                          (float) 6.0536496345054e-3, (float) 9.88555033724111e-4, (float) 3.64943550840577e-5,
+                          (float) 1.55942290996993e-5);
+    float denom = poly7(x2, 1.f, (float) 7.58517175815194e-1, (float) 2.81364355593059e-1, (float) 6.81783097841267e-2,
+                            (float) 1.13586116798019e-2, (float) 1.92020805811771e-3, (float) 5.74217664074868e-5,
+                            (float) 3.11884331363595e-5);
+    return fmul(__fdiv_rn(num, denom), x);
+}
+
+/* special.h:267-271 erfi = M_2_SQRTPI * dawson(x) * exp(x * x) */
+__device__ __forceinline__ float erfi_f32(float x) {
+    return fmul(fmul((float) 1.12837916709551257390, dawson_f32(x)), exp_f32(fmul(x, x)));
+}
+
 /* ---------------- two elements at a time ----------------
    The sweep kernels evaluate exp / sin / cos on pairs of elements: the two independent dependency chains give
    ptxas instruction-level parallelism to interleave.  sm_90 has no packed fp32 arithmetic, so every pair

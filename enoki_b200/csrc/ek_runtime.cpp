@@ -53,7 +53,7 @@ const char *ek_op_name(ek_op op) {
         "and", "or", "xor", "gt", "ge", "lt", "le", "eq", "ne", "mul_nz", "fma", "select", "fma_nz",
         "gather", "scatter", "scatter_add", "hsum", "hprod", "hmax", "hmin", "all", "any", "count", "printf",
         "tan", "cot", "asin", "acos", "atan", "atan2", "sinh", "cosh", "tanh", "asinh", "acosh", "atanh", "cbrt",
-        "erf", "erfc", "erfinv", "lgamma", "tgamma" };
+        "erf", "erfc", "erfinv", "lgamma", "tgamma", "pow", "frexp_m", "frexp_e", "hypot", "dawson", "erfi" };
     return (unsigned) op < EK_OP__COUNT ? names[op] : "?";
 }
 

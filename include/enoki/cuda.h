@@ -245,6 +245,20 @@ struct CUDAArray : ArrayBase<value_t<Value>, CUDAArray<Value>> {
     template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray erfinv_() const { return un_(EK_OP_ERFINV); }
     template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray lgamma_() const { return un_(EK_OP_LGAMMA); }
     template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray tgamma_() const { return un_(EK_OP_TGAMMA); }
+    /// pow/frexp: the same for array_math.h:682-709,956-958.  pow(x, y) with a scalar y that is an integer keeps
+    /// array_math.h's repeated multiplication; any other y reaches pow_.  fmod and ldexp keep their traced bodies: on an
+    /// H100 their native forms measured no faster (DESIGN.md 6).
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0>
+    CUDAArray pow_(const CUDAArray &y) const { return bin_(EK_OP_POW, y); }
+    /// frexp(*this): (mantissa, exponent), two nodes
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0>
+    std::pair<CUDAArray, CUDAArray> frexp_() const { return { un_(EK_OP_FREXP_M), un_(EK_OP_FREXP_E) }; }
+    /// hypot/dawson/erfi: called by the free overloads of CUDAArray<float> below (array_math.h:1362-1379,
+    /// special.h:249-271)
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0>
+    CUDAArray hypot_(const CUDAArray &b) const { return bin_(EK_OP_HYPOT, b); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray dawson_() const { return un_(EK_OP_DAWSON); }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray erfi_() const { return un_(EK_OP_ERFI); }
     CUDAArray floor_() const { return un_(EK_OP_FLOOR); }
     CUDAArray ceil_() const { return un_(EK_OP_CEIL); }
     CUDAArray round_() const { return un_(EK_OP_ROUND); }
@@ -488,6 +502,12 @@ inline CUDAArray<float> erfc(const CUDAArray<float> &x) { return x.erfc_(); }
 inline CUDAArray<float> erfinv(const CUDAArray<float> &x) { return x.erfinv_(); }
 inline CUDAArray<float> lgamma(const CUDAArray<float> &x) { return x.lgamma_(); }
 inline CUDAArray<float> tgamma(const CUDAArray<float> &x) { return x.tgamma_(); }
+/// The same for array_math.h's free template hypot and special.h's dawson and erfi.  Only a call whose operands are all
+/// CUDAArray<float> matches: a mixed call such as hypot(x, 1.f) still takes array_math.h's template and records its body
+/// op by op.  erfi<FloatC>(x) calls dawson unqualified, so its traced body uses the native dawson.
+inline CUDAArray<float> hypot(const CUDAArray<float> &a, const CUDAArray<float> &b) { return a.hypot_(b); }
+inline CUDAArray<float> dawson(const CUDAArray<float> &x) { return x.dawson_(); }
+inline CUDAArray<float> erfi(const CUDAArray<float> &x) { return x.erfi_(); }
 
 template <typename T, enable_if_t<!is_diff_array_v<T> && is_cuda_array_v<T>> = 0>
 ENOKI_INLINE void set_label(const T &a, const char *label) {

@@ -137,6 +137,12 @@ typedef enum ek_op {
     EK_OP_ERFINV,      /* special.h:222-246 */
     EK_OP_LGAMMA,      /* special.h:275-309 */
     EK_OP_TGAMMA,      /* special.h:312     exp(lgamma(x))                                  */
+    EK_OP_POW,         /* array_math.h:956-958  exp(log(x) * y), operands (x, y)            */
+    EK_OP_FREXP_M,     /* array_math.h:682-709  frexp(x).first: the mantissa                */
+    EK_OP_FREXP_E,     /* array_math.h:682-709  frexp(x).second: the exponent, as a float   */
+    EK_OP_HYPOT,       /* array_math.h:1362-1379  operands (a, b)                           */
+    EK_OP_DAWSON,      /* special.h:249-265 */
+    EK_OP_ERFI,        /* special.h:267-271  M_2_SQRTPI * dawson(x) * exp(x * x)            */
     EK_OP__COUNT
 } ek_op;
 
