@@ -32,7 +32,10 @@ OP = {n: i for i, n in enumerate(_OPS + _OPS_SPECIAL)}
 # EK_FX_MATH); a table of their own, so that OP keeps the opcodes it held before they existed
 _OPS_MATH = ["POW", "FREXP_M", "FREXP_E", "HYPOT", "DAWSON", "ERFI"]
 OP_MATH = {n: len(OP) + i for i, n in enumerate(_OPS_MATH)}
-_OPCODE = {**OP, **OP_MATH}
+# special.h's Carlson integrals, numbered after EK_OP_ERFI (their sweep operations: EK_FX_ELL), in a table of their own
+_OPS_ELL = ["CARLSON_RF", "CARLSON_RD", "CARLSON_RC"]
+OP_ELL = {n: len(OP) + len(OP_MATH) + i for i, n in enumerate(_OPS_ELL)}
+_OPCODE = {**OP, **OP_MATH, **OP_ELL}
 
 _NP = {EK_INT8: np.int8, EK_UINT8: np.uint8, EK_INT16: np.int16, EK_UINT16: np.uint16,
        EK_INT32: np.int32, EK_UINT32: np.uint32, EK_INT64: np.int64, EK_UINT64: np.uint64,
@@ -291,6 +294,45 @@ hypot = _binary("HYPOT", "hypot(a, b) (array_math.h:1362-1379); either operand m
 def frexp(x):
     """(mantissa, exponent) of array_math.h:682-709, both Float32"""
     return x._un("FREXP_M"), x._un("FREXP_E")
+
+
+def _operands(*args):
+    """the arguments as arrays of the first array argument's type (Float32 when all are Python numbers)"""
+    cls = next((type(v) for v in args if isinstance(v, CUDAArray)), Float32)
+    return [v if isinstance(v, CUDAArray) else cls(v) for v in args]
+
+
+# Float32 only: one node each, bit for bit the single precision bodies of special.h, their duplication loops run per
+# element on the device (DESIGN.md 4); any argument may be a Python number.  No autodiff: the reference has no
+# derivatives for them.
+def carlson_rf(x, y, z):
+    """R_F(x, y, z) (special.h:325-366)"""
+    x, y, z = _operands(x, y, z)
+    return type(x).from_index(_append(x.Type, "CARLSON_RF", x.index, y.index, z.index))
+
+
+def carlson_rd(x, y, z):
+    """R_D(x, y, z) (special.h:379-432)"""
+    x, y, z = _operands(x, y, z)
+    return type(x).from_index(_append(x.Type, "CARLSON_RD", x.index, y.index, z.index))
+
+
+def carlson_rc(x, y):
+    """R_C(x, y) (special.h:445-482)"""
+    x, y = _operands(x, y)
+    return x._bin("CARLSON_RC", y)
+
+
+def comp_ellint_1(k):
+    """K(k) = carlson_rf(0, 1 - k^2, 1) (special.h:566-572): k is squared, unlike Mathematica's EllipticK"""
+    return carlson_rf(0.0, 1.0 - k * k, 1.0)
+
+
+def comp_ellint_2(k):
+    """E(k) = carlson_rf(xyz) - 1/3 k^2 carlson_rd(xyz), xyz = (0, 1 - k^2, 1) (special.h:599-606)"""
+    k2 = k * k
+    y = 1.0 - k2
+    return carlson_rf(0.0, y, 1.0) - (1.0 / 3.0) * k2 * carlson_rd(0.0, y, 1.0)
 
 
 def sincos(x):

@@ -166,6 +166,9 @@ int pick_op(ek_op op, ek_type vt, ek_type at /* operand type */) {
         case EK_OP_HYPOT:   return SEL(DOP_HYPOT_F32, -1, -1, -1, -1, -1);
         case EK_OP_DAWSON:  return SEL(DOP_DAWSON_F32, -1, -1, -1, -1, -1);
         case EK_OP_ERFI:    return SEL(DOP_ERFI_F32, -1, -1, -1, -1, -1);
+        case EK_OP_CARLSON_RF: return SEL(DOP_CARLSON_RF_F32, -1, -1, -1, -1, -1);
+        case EK_OP_CARLSON_RD: return SEL(DOP_CARLSON_RD_F32, -1, -1, -1, -1, -1);
+        case EK_OP_CARLSON_RC: return SEL(DOP_CARLSON_RC_F32, -1, -1, -1, -1, -1);
         case EK_OP_FLOOR: return SEL(DOP_FLOOR_F32, DOP_FLOOR_F64, DOP_LOAD_32, DOP_LOAD_32, DOP_LOAD_64, DOP_LOAD_64);
         case EK_OP_CEIL:  return SEL(DOP_CEIL_F32, DOP_CEIL_F64, DOP_LOAD_32, DOP_LOAD_32, DOP_LOAD_64, DOP_LOAD_64);
         case EK_OP_ROUND: return SEL(DOP_ROUND_F32, DOP_ROUND_F64, DOP_LOAD_32, DOP_LOAD_32, DOP_LOAD_64, DOP_LOAD_64);
@@ -244,6 +247,7 @@ uint32_t acc_positions(const EkVariable &v) {
     if (ek_op_unary(op)) return 1;
     if (ek_op_binary(op)) return 3;
     if (op == EK_OP_FMA || op == EK_OP_SELECT || op == EK_OP_FMA_NZ) return 7;
+    if (ek_op_carlson3(op)) return 1;
     if (op == EK_OP_GATHER || op == EK_OP_SCATTER || op == EK_OP_SCATTER_ADD) return 2;   /* the index */
     if (op >= EK_OP_HSUM && op <= EK_OP_COUNT) return 1;
     return 0;
@@ -889,6 +893,14 @@ struct Assembler {
                 else if (p == 1) { put_b(in, d0); put_c(in, d2); }
                 else { put_b(in, d0); put_c(in, d1); }
             } break;
+            case EK_OP_CARLSON_RF: case EK_OP_CARLSON_RD: {
+                /* x is the accumulator (acc_positions): when it holds y or z, x is loaded by the instruction itself */
+                int dop = pick_op(op, t, var(d0).type);
+                if (dop < 0) return fail(std::string("op ") + ek_op_name(op) + " not supported for type " + ek_type_name(t));
+                ensure_acc(d0);
+                in = mk(dop);
+                put_b(in, d1); put_c(in, d2);
+            } break;
             case EK_OP_AND: case EK_OP_OR: {
                 ek_type bt = var(d1).type;
                 if (t != EK_BOOL && bt == EK_BOOL) {
@@ -928,7 +940,7 @@ struct Assembler {
                             case EK_OP_LT: eop = EK_OP_GT; break;
                             case EK_OP_LE: eop = EK_OP_GE; break;
                             case EK_OP_SUB: case EK_OP_DIV: case EK_OP_MOD: case EK_OP_SHL: case EK_OP_SHR: case EK_OP_ATAN2:
-                            case EK_OP_POW: case EK_OP_HYPOT: reversed = true; break;
+                            case EK_OP_POW: case EK_OP_HYPOT: case EK_OP_CARLSON_RC: reversed = true; break;
                             case EK_OP_MIN: case EK_OP_MAX: reversed = ek_is_float(t); break;
                             default: break;       /* commutative */
                         }
@@ -1048,6 +1060,7 @@ struct Assembler {
         switch (dop) {
             case DOP_SUB_F32: return DOP_SUBR_F32; case DOP_DIV_F32: return DOP_DIVR_F32; case DOP_ATAN2_F32: return DOP_ATAN2R_F32;
             case DOP_POW_F32: return DOP_POWR_F32; case DOP_HYPOT_F32: return DOP_HYPOTR_F32;
+            case DOP_CARLSON_RC_F32: return DOP_CARLSON_RCR_F32;
             case DOP_MIN_F32: return DOP_MINR_F32; case DOP_MAX_F32: return DOP_MAXR_F32;
             case DOP_SUB_F64: return DOP_SUBR_F64; case DOP_DIV_F64: return DOP_DIVR_F64;
             case DOP_MIN_F64: return DOP_MINR_F64; case DOP_MAX_F64: return DOP_MAXR_F64;
@@ -1101,6 +1114,8 @@ struct Assembler {
                              case DOP_HYPOT_F32: case DOP_HYPOTR_F32: return 8.0;
                              case DOP_DAWSON_F32: return 6.0;
                              case DOP_ERFI_F32: return 14.0;
+                             case DOP_CARLSON_RF_F32: case DOP_CARLSON_RD_F32: return 60.0;
+                             case DOP_CARLSON_RC_F32: case DOP_CARLSON_RCR_F32: return 40.0;
                              case DOP_SQRT_F32: case DOP_DIV_F32: case DOP_RCP_F32: case DOP_RSQRT_F32: return 3.0; default: return 1.0; } };
         double total_w = 0; for (const EkInstr &in : out.body) total_w += weight(in);
         double acc_w = 0;
@@ -1321,6 +1336,7 @@ int fop_of(int dop) {
         X(SINH_F32) X(COSH_F32) X(TANH_F32) X(ASINH_F32) X(ACOSH_F32) X(ATANH_F32) X(CBRT_F32)
         X(ERF_F32) X(ERFC_F32) X(ERFINV_F32) X(LGAMMA_F32) X(TGAMMA_F32)
         X(POW_F32) X(POWR_F32) X(FREXP_M_F32) X(FREXP_E_F32) X(HYPOT_F32) X(HYPOTR_F32) X(DAWSON_F32) X(ERFI_F32)
+        X(CARLSON_RF_F32) X(CARLSON_RD_F32) X(CARLSON_RC_F32) X(CARLSON_RCR_F32)
 #undef X
         case DOP_LOAD_32: return FOP_LOAD;
         default: return -1;
@@ -1826,7 +1842,7 @@ void write_program_json(std::ostream &os, const EkContext &ctx, const std::vecto
             EK_FOPS2(X)
 #undef X
 #define X(n) #n,
-            EK_FOPS1(X) EK_FOPS0(X) EK_FOPS16(X) EK_FOPST(X) EK_FOPSH(X) EK_FOPSS(X) EK_FOPSM(X)
+            EK_FOPS1(X) EK_FOPS0(X) EK_FOPS16(X) EK_FOPST(X) EK_FOPSH(X) EK_FOPSS(X) EK_FOPSM(X) EK_FOPSE(X)
 #undef X
         };
         for (int k = 0; k < FOP__COUNT; ++k) os << (k ? "," : "") << "\"" << fnames[k] << "\"";
@@ -1928,7 +1944,7 @@ bool launch_sweep(EkContext &ctx, const Sweep &s) {
     if (cfg.fast) {
         ek_cuda_check(ek_launch_sweep_fast(args, grid, cfg.T, cfg.smem, ctx.stream));
     } else {
-        bool trig = false;          /* the general kernel's instantiation with the trigonometric, hyperbolic, special and other math operations */
+        bool trig = false;          /* the general kernel's instantiation with the trigonometric, hyperbolic, special, other math and Carlson operations */
         for (const EkInstr &in : a.body) trig |= ek_dop_ext(in.op);
         ek_cuda_check(ek_launch_sweep(cfg.V, inline_prog, trig, args, grid, cfg.T, cfg.smem, ctx.stream));
     }

@@ -102,7 +102,7 @@ void ek_cuda_check_impl(cudaError_t err, const char *file, int line);
 #define ek_cuda_check(x) ek_cuda_check_impl((x), __FILE__, __LINE__)
 
 /* kernels (defined in .cu files) */
-/* trig: the body contains an operation of the extension instantiations (ek_isa.h ek_dop_ext: tan ... erfi) */
+/* trig: the body contains an operation of the extension instantiations (ek_isa.h ek_dop_ext: tan ... carlson_rc) */
 cudaError_t ek_launch_sweep(int V, bool inline_prog, bool trig, const EkSweepArgs &args, unsigned grid, unsigned block,
                             size_t smem_bytes, cudaStream_t stream);
 /* 32-bit fast kernel (ek_sweep_fast.cu): args.prog_inline holds the lowered program; block = 128 or 256 */
@@ -137,8 +137,11 @@ static inline bool ek_op_unary(ek_op op) {
            op == EK_OP_FREXP_M || op == EK_OP_FREXP_E || op == EK_OP_DAWSON || op == EK_OP_ERFI;
 }
 static inline bool ek_op_binary(ek_op op) {
-    return (op >= EK_OP_ADD && op <= EK_OP_MUL_NZ) || op == EK_OP_ATAN2 || op == EK_OP_POW || op == EK_OP_HYPOT;
+    return (op >= EK_OP_ADD && op <= EK_OP_MUL_NZ) || op == EK_OP_ATAN2 || op == EK_OP_POW || op == EK_OP_HYPOT ||
+           op == EK_OP_CARLSON_RC;
 }
+/* the ternary Carlson integrals (x, y, z): only x is read from the accumulator */
+static inline bool ek_op_carlson3(ek_op op) { return op == EK_OP_CARLSON_RF || op == EK_OP_CARLSON_RD; }
 
 /* cuda_printf formats (ek_printf.cpp).  A parsed format is a list of segments: literal text (conv == 0, "%%" already
    reduced to "%") or one conversion, `text` being its spec as written ("%-08.3lx") and `arg` the argument it takes. */

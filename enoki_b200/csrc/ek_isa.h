@@ -141,7 +141,9 @@ struct EkInstr {
     X(SINH_F32) X(COSH_F32) X(TANH_F32) X(ASINH_F32) X(ACOSH_F32) X(ATANH_F32) X(CBRT_F32) \
     X(ERF_F32) X(ERFC_F32) X(ERFINV_F32) X(LGAMMA_F32) X(TGAMMA_F32) \
     /* further f32 functions of array_math.h and special.h; POW / HYPOT: R = x, B = y, POWR / HYPOTR: R = y, B = x */ \
-    X(POW_F32) X(POWR_F32) X(FREXP_M_F32) X(FREXP_E_F32) X(HYPOT_F32) X(HYPOTR_F32) X(DAWSON_F32) X(ERFI_F32)
+    X(POW_F32) X(POWR_F32) X(FREXP_M_F32) X(FREXP_E_F32) X(HYPOT_F32) X(HYPOTR_F32) X(DAWSON_F32) X(ERFI_F32) \
+    /* Carlson integrals of special.h; RF / RD: R = x, B = y, C = z; RC: R = x, B = y, RCR: R = y, B = x */ \
+    X(CARLSON_RF_F32) X(CARLSON_RD_F32) X(CARLSON_RC_F32) X(CARLSON_RCR_F32)
 
 enum EkDop : uint16_t {
 #define X(n) DOP_##n,
@@ -151,7 +153,7 @@ enum EkDop : uint16_t {
 };
 
 /* the operations that only the extension instantiations of the sweep kernels carry (ek_sweep_kernel<V, INLINE, true>;
-   lowered, ek_fast_kernel<T, EK_FX_TRIG / EK_FX_HYP / EK_FX_SPEC / EK_FX_MATH>): tan ... erfi, numbered after every other
+   lowered, ek_fast_kernel<T, EK_FX_TRIG / EK_FX_HYP / EK_FX_SPEC / EK_FX_MATH / EK_FX_ELL>): tan ... carlson_rc, numbered after every other
    operation.  The imm field of these instructions is free, and a body that contains one runs on those instantiations. */
 static inline bool ek_dop_ext(uint32_t op) { return op >= DOP_TAN_F32 && op < DOP__COUNT; }
 
@@ -216,6 +218,9 @@ static inline bool ek_dop_ext(uint32_t op) { return op >= DOP_TAN_F32 && op < DO
    FMA_F32_UB) */
 #define EK_FOPSM(X) X(POW_F32) X(POW_F32_UB) X(POWR_F32) X(POWR_F32_UB) X(FREXP_M_F32) X(FREXP_E_F32) \
                     X(HYPOT_F32) X(HYPOT_F32_UB) X(HYPOTR_F32) X(HYPOTR_F32_UB) X(DAWSON_F32) X(ERFI_F32)
+/* carlson_rf, carlson_rd and carlson_rc, in the bodies that the EK_FX_ELL instantiations run (numbered last).  The
+   accumulator is x (RCR: y); no uniform twins: a literal or scalar operand is broadcast (FF_BU / FF_CU) */
+#define EK_FOPSE(X) X(CARLSON_RF_F32) X(CARLSON_RD_F32) X(CARLSON_RC_F32) X(CARLSON_RCR_F32)
 
 /* feature bits of the ek_fast_kernel instantiations: the launcher runs the smallest one whose operations cover the
    lowered body */
@@ -224,7 +229,8 @@ static inline bool ek_dop_ext(uint32_t op) { return op >= DOP_TAN_F32 && op < DO
 #define EK_FX_HYP  4u     /* EK_FOPSH */
 #define EK_FX_SPEC 8u     /* EK_FOPSS */
 #define EK_FX_MATH 16u    /* EK_FOPSM */
-#define EK_FX_ALL  (EK_FX_F16 | EK_FX_TRIG | EK_FX_HYP | EK_FX_SPEC | EK_FX_MATH)
+#define EK_FX_ELL  32u    /* EK_FOPSE */
+#define EK_FX_ALL  (EK_FX_F16 | EK_FX_TRIG | EK_FX_HYP | EK_FX_SPEC | EK_FX_MATH | EK_FX_ELL)
 
 enum EkFop : uint16_t {
     FOP_NOP,
@@ -239,6 +245,7 @@ enum EkFop : uint16_t {
     EK_FOPSH(X)
     EK_FOPSS(X)
     EK_FOPSM(X)
+    EK_FOPSE(X)
 #undef X
     FOP__COUNT
 };
@@ -249,7 +256,8 @@ static inline uint32_t ek_fast_ext(const EkInstr *body, uint32_t n) {
     for (uint32_t pc = 0; pc < n; ++pc) {
         const uint32_t op = body[pc].op;
         if (op == FOP_LD_F16 || op == FOP_ST_F16) ext |= EK_FX_F16;
-        else if (op >= FOP_POW_F32 && op < FOP__COUNT) ext |= EK_FX_MATH;
+        else if (op >= FOP_CARLSON_RF_F32 && op < FOP__COUNT) ext |= EK_FX_ELL;
+        else if (op >= FOP_POW_F32 && op <= FOP_ERFI_F32) ext |= EK_FX_MATH;
         else if (op >= FOP_ERF_F32 && op <= FOP_TGAMMA_F32) ext |= EK_FX_SPEC;
         else if (op >= FOP_SINH_F32 && op <= FOP_CBRT_F32) ext |= EK_FX_HYP;
         else if (op >= FOP_TAN_F32) ext |= EK_FX_TRIG;

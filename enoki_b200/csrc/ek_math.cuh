@@ -444,6 +444,84 @@ __device__ __forceinline__ float erfi_f32(float x) {
     return fmul(fmul((float) 1.12837916709551257390, dawson_f32(x)), exp_f32(fmul(x, x)));
 }
 
+/* ---------------- carlson_rf, carlson_rd, carlson_rc ----------------
+   The single precision bodies of special.h's Carlson integrals, one element at a time.  special.h runs their
+   duplication loop on the host over whole arrays: every update is masked by `active`, which only ever turns off, and the
+   loop ends when no element is active or after the tenth evaluation of the loop head.  An element that has stopped keeps
+   its arguments, so each later pass recomputes the same XYZ and mu_inv for it; element by element the loop is therefore
+   "evaluate the head; stop if !(eps > threshold) or this was the tenth head; update", which is what these loops do.
+   The operations are the recorded ones: correctly rounded sqrt, rcp and division; dot() of a nested array as
+   array_static.h:948-958's product and fmadd chain; hsum / hprod / hmax as left folds, hmax with the x86 max rule;
+   fnmadd as one fma; masked updates as selects; constants and thresholds rounded to float as Scalar(c) rounds them. */
+
+/* special.h:325-366 carlson_rf(x, y, z) */
+__device__ __forceinline__ float carlson_rf_f32(float x, float y, float z) {
+    const float thr = (float) 0.070154;
+    float X, Y, Z, mu_inv;
+#pragma unroll 1
+    for (int it = 1;; ++it) {
+        const float sx = __fsqrt_rn(x), sy = __fsqrt_rn(y), sz = __fsqrt_rn(z);
+        const float lambda = ffma(sx, sz, ffma(sz, sy, fmul(sy, sx)));          /* dot(shuffle<1, 2, 0>(s), s) */
+        const float mu = fmul(fadd(fadd(x, y), z), (float) (1.0 / 3.0));
+        mu_inv = __frcp_rn(mu);
+        X = ffma(-x, mu_inv, 1.f); Y = ffma(-y, mu_inv, 1.f); Z = ffma(-z, mu_inv, 1.f);
+        const float eps = max_x86(max_x86(fabsf(X), fabsf(Y)), fabsf(Z));
+        if (!(eps > thr) || it == 10) break;
+        x = fmul(fadd(x, lambda), 0.25f); y = fmul(fadd(y, lambda), 0.25f); z = fmul(fadd(z, lambda), 0.25f);
+    }
+    const float e2 = fsub(fmul(X, Y), fmul(Z, Z)), e3 = fmul(fmul(X, Y), Z);
+    const float er = fadd(fmul(fsub(fsub(fmul((float) (1.0 / 24.0), e2), (float) (1.0 / 10.0)),
+                                    fmul((float) (3.0 / 44.0), e3)), e2),
+                          fmul((float) (1.0 / 14.0), e3));
+    return fmul(__fsqrt_rn(mu_inv), fadd(1.f, er));
+}
+
+/* special.h:379-432 carlson_rd(x, y, z) */
+__device__ __forceinline__ float carlson_rd_f32(float x, float y, float z) {
+    const float thr = (float) (0.070154 * 0.6);
+    const float w0 = (float) (1.0 / 5.0), w2 = (float) (3.0 / 5.0);
+    float X, Y, Z, mu_inv, sum = 0.f, num = 1.f;
+#pragma unroll 1
+    for (int it = 1;; ++it) {
+        const float sx = __fsqrt_rn(x), sy = __fsqrt_rn(y), sz = __fsqrt_rn(z);
+        const float lambda = ffma(sx, sz, ffma(sz, sy, fmul(sy, sx)));
+        const float mu = fadd(fadd(fmul(x, w0), fmul(y, w0)), fmul(z, w2));     /* hsum(xyz * W) */
+        mu_inv = __frcp_rn(mu);
+        X = ffma(-x, mu_inv, 1.f); Y = ffma(-y, mu_inv, 1.f); Z = ffma(-z, mu_inv, 1.f);
+        const float eps = max_x86(max_x86(fabsf(X), fabsf(Y)), fabsf(Z));
+        if (!(eps > thr) || it == 10) break;
+        sum = fadd(sum, __fdiv_rn(num, fmul(sz, fadd(z, lambda))));
+        num = fmul(num, 0.25f);
+        x = fmul(fadd(x, lambda), 0.25f); y = fmul(fadd(y, lambda), 0.25f); z = fmul(fadd(z, lambda), 0.25f);
+    }
+    const float ea = fmul(X, Y), eb = fmul(Z, Z), ec = fsub(ea, eb);
+    const float ed = ffma(-6.f, eb, ea), ee = ffma(ec, 2.f, ed);
+    const float p1 = fmul(ed, fsub(fadd(-(float) (3.0 / 14.0), fmul((float) (9.0 / 88.0), ed)),
+                                   fmul(fmul(0.25f, Z), ee)));
+    const float p2 = fmul(Z, fadd(fmul((float) (1.0 / 6.0), ee),
+                                  fmul(Z, fadd(fmul(-(float) (9.0 / 22.0), ec), fmul(fmul(Z, (float) (3.0 / 26.0)), ea)))));
+    const float p = fadd(p1, p2);
+    return fadd(fmul(3.f, sum), fmul(fmul(fmul(num, mu_inv), __fsqrt_rn(mu_inv)), fadd(1.f, p)));
+}
+
+/* special.h:445-482 carlson_rc(x, y); lambda += lambda + y rounds twice */
+__device__ __forceinline__ float carlson_rc_f32(float x, float y) {
+    const float thr = (float) (0.070154 * 0.48);
+    float inv_mu, s;
+#pragma unroll 1
+    for (int it = 1;; ++it) {
+        float lambda = fmul(__fsqrt_rn(x), __fsqrt_rn(y));
+        lambda = fadd(lambda, fadd(lambda, y));
+        const float mu = ffma(x, (float) (1.0 / 3.0), fmul(y, (float) (2.0 / 3.0)));
+        inv_mu = __frcp_rn(mu);
+        s = fmul(fsub(y, mu), inv_mu);
+        if (!(fabsf(s) > thr) || it == 10) break;
+        x = fmul(fadd(x, lambda), 0.25f); y = fmul(fadd(y, lambda), 0.25f);
+    }
+    const float q = fadd(0.3f, fmul(s, fadd((float) (1.0 / 7.0), fmul(s, fadd(0.375f, fmul(s, (float) (9.0 / 22.0)))))));
+    return fmul(__fsqrt_rn(inv_mu), fadd(1.f, fmul(fmul(s, s), q)));
+}
+
 /* ---------------- two elements at a time ----------------
    The sweep kernels evaluate exp / sin / cos on pairs of elements: the two independent dependency chains give
    ptxas instruction-level parallelism to interleave.  sm_90 has no packed fp32 arithmetic, so every pair

@@ -53,7 +53,8 @@ const char *ek_op_name(ek_op op) {
         "and", "or", "xor", "gt", "ge", "lt", "le", "eq", "ne", "mul_nz", "fma", "select", "fma_nz",
         "gather", "scatter", "scatter_add", "hsum", "hprod", "hmax", "hmin", "all", "any", "count", "printf",
         "tan", "cot", "asin", "acos", "atan", "atan2", "sinh", "cosh", "tanh", "asinh", "acosh", "atanh", "cbrt",
-        "erf", "erfc", "erfinv", "lgamma", "tgamma", "pow", "frexp_m", "frexp_e", "hypot", "dawson", "erfi" };
+        "erf", "erfc", "erfinv", "lgamma", "tgamma", "pow", "frexp_m", "frexp_e", "hypot", "dawson", "erfi",
+        "carlson_rf", "carlson_rd", "carlson_rc" };
     return (unsigned) op < EK_OP__COUNT ? names[op] : "?";
 }
 
@@ -465,7 +466,7 @@ static int op_arity(ek_op op) {
     if (op == EK_OP_LITERAL || op == EK_OP_INDEX) return 0;
     if (ek_op_unary(op)) return 1;
     if (ek_op_binary(op)) return 2;
-    if (op == EK_OP_FMA || op == EK_OP_SELECT || op == EK_OP_FMA_NZ) return 3;
+    if (op == EK_OP_FMA || op == EK_OP_SELECT || op == EK_OP_FMA_NZ || ek_op_carlson3(op)) return 3;
     if (op == EK_OP_GATHER || op == EK_OP_SCATTER || op == EK_OP_SCATTER_ADD) return 3;
     if (op >= EK_OP_HSUM && op <= EK_OP_COUNT) return 1;
     return -1;

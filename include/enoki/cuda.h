@@ -259,6 +259,18 @@ struct CUDAArray : ArrayBase<value_t<Value>, CUDAArray<Value>> {
     CUDAArray hypot_(const CUDAArray &b) const { return bin_(EK_OP_HYPOT, b); }
     template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray dawson_() const { return un_(EK_OP_DAWSON); }
     template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0> CUDAArray erfi_() const { return un_(EK_OP_ERFI); }
+    /// carlson_rf/carlson_rd/carlson_rc with *this as x: called by the free overloads of Array<CUDAArray<float>, N>
+    /// below (special.h:325-482)
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0>
+    CUDAArray carlson_rf_(const CUDAArray &y, const CUDAArray &z) const {
+        return from_index_(detail::ek_append(Type, EK_OP_CARLSON_RF, m_index, y.m_index, z.m_index));
+    }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0>
+    CUDAArray carlson_rd_(const CUDAArray &y, const CUDAArray &z) const {
+        return from_index_(detail::ek_append(Type, EK_OP_CARLSON_RD, m_index, y.m_index, z.m_index));
+    }
+    template <typename T = Value, enable_if_t<std::is_same_v<T, float>> = 0>
+    CUDAArray carlson_rc_(const CUDAArray &y) const { return bin_(EK_OP_CARLSON_RC, y); }
     CUDAArray floor_() const { return un_(EK_OP_FLOOR); }
     CUDAArray ceil_() const { return un_(EK_OP_CEIL); }
     CUDAArray round_() const { return un_(EK_OP_ROUND); }
@@ -508,6 +520,16 @@ inline CUDAArray<float> tgamma(const CUDAArray<float> &x) { return x.tgamma_(); 
 inline CUDAArray<float> hypot(const CUDAArray<float> &a, const CUDAArray<float> &b) { return a.hypot_(b); }
 inline CUDAArray<float> dawson(const CUDAArray<float> &x) { return x.dawson_(); }
 inline CUDAArray<float> erfi(const CUDAArray<float> &x) { return x.erfi_(); }
+/// special.h's Carlson integrals take one vector: these overloads match exactly Array<CUDAArray<float>, 3> (carlson_rf,
+/// carlson_rd) and Array<CUDAArray<float>, 2> (carlson_rc), which is what comp_ellint_1/2 and ellint_1/2 build and what
+/// carlson_rj passes to carlson_rc, so those pick them up.  Each is one node: the duplication loop runs per element on
+/// the device instead of on the host with one synchronisation per pass (DESIGN.md 4).  The templates' assert on the
+/// argument domain is not evaluated here (it would cost an evaluation and a synchronisation of its own); arguments
+/// outside it give what the traced body gives.  DiffArray, CUDAArray<double>, types derived from Array and calls with
+/// explicit template arguments keep the templates.
+inline CUDAArray<float> carlson_rf(const Array<CUDAArray<float>, 3> &xyz) { return xyz.x().carlson_rf_(xyz.y(), xyz.z()); }
+inline CUDAArray<float> carlson_rd(const Array<CUDAArray<float>, 3> &xyz) { return xyz.x().carlson_rd_(xyz.y(), xyz.z()); }
+inline CUDAArray<float> carlson_rc(const Array<CUDAArray<float>, 2> &xy) { return xy.x().carlson_rc_(xy.y()); }
 
 template <typename T, enable_if_t<!is_diff_array_v<T> && is_cuda_array_v<T>> = 0>
 ENOKI_INLINE void set_label(const T &a, const char *label) {

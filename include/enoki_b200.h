@@ -143,6 +143,9 @@ typedef enum ek_op {
     EK_OP_HYPOT,       /* array_math.h:1362-1379  operands (a, b)                           */
     EK_OP_DAWSON,      /* special.h:249-265 */
     EK_OP_ERFI,        /* special.h:267-271  M_2_SQRTPI * dawson(x) * exp(x * x)            */
+    EK_OP_CARLSON_RF,  /* special.h:325-366  carlson_rf(x, y, z), operands (x, y, z)         */
+    EK_OP_CARLSON_RD,  /* special.h:379-432  carlson_rd(x, y, z), operands (x, y, z)         */
+    EK_OP_CARLSON_RC,  /* special.h:445-482  carlson_rc(x, y), operands (x, y)               */
     EK_OP__COUNT
 } ek_op;
 
