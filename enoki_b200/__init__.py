@@ -527,3 +527,4 @@ def device_count():
 
 
 from .autodiff import FloatD, backward, forward, gradient, set_requires_gradient, detach  # noqa: E402,F401
+from .dlpack import from_dlpack  # noqa: E402,F401  (also installs __dlpack__ / __dlpack_device__ / from_dlpack)

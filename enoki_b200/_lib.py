@@ -88,6 +88,11 @@ SIGNATURES = {
     "ek_memcpy_from_device_async": (None, [c_vp, c_vp, c_sz]),
     "ek_memcpy_from_device_overlapped": (None, [c_vp, c_vp, c_sz]),
     "ek_memcpy_device_async": (None, [c_vp, c_vp, c_sz]),
+    "ek_dlpack_export": (c_vp, [c_u32, c_int, c_vp]),
+    "ek_dlpack_import": (c_u32, [c_vp, c_int]),
+    "ek_device": (c_int, []),
+    "ek_stream_wait_external": (c_int, [c_vp]),
+    "ek_stream_signal_external": (c_int, [c_vp]),
     "ek_tape_append_node": (c_u32, [c_int, c_sz, ctypes.c_char_p]),
     "ek_tape_append_leaf": (c_u32, [c_int, c_sz]),
     "ek_tape_append_edge": (c_int, [c_int, c_u32, c_u32, c_u32]),

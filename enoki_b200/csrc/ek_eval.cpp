@@ -2120,6 +2120,7 @@ void dump_prints(std::ostream &os, const EkContext &ctx, const std::vector<uint3
 extern "C" {
 
 int ek_eval(void) {
+    ek_dlpack_drain();
     EkContext &ctx = ek_ctx();
     for (auto cb : ctx.callbacks) cb.first(cb.second);         /* jit.cu:1421-1422 */
     if (ctx.live.empty()) { clear_dirty(ctx); return 0; }

@@ -14,6 +14,7 @@
 #include <map>
 #include <unordered_map>
 #include <memory>
+#include <atomic>
 #include "../../include/enoki_b200.h"
 #include "ek_isa.h"
 
@@ -37,6 +38,8 @@ struct EkVariable {
     bool used = false;                  /* slot in use */
     std::string *label = nullptr;
     std::string *fmt = nullptr;         /* format of a print node (EK_OP_PRINTF), owned with it */
+    void *dlpack = nullptr;             /* imported DLPack tensor that owns `data` (ek_dlpack.cpp); free_data is false */
+    bool dlpack_versioned = false;
 };
 
 struct EkProgramCacheEntry {
@@ -70,6 +73,7 @@ struct EkContext {
        allocator synchronises and trims, because that work may still read blocks on the free list */
     cudaStream_t d2h_stream = nullptr;          /* read-back stream of ek_memcpy_from_device_overlapped() */
     cudaEvent_t d2h_event = nullptr;
+    cudaEvent_t handoff_event = nullptr;        /* ek_stream_wait_external / ek_stream_signal_external */
     void (*pre_trim_hook)(void *) = nullptr;
     void *pre_trim_arg = nullptr;
 
@@ -100,6 +104,21 @@ EkContext &ek_ctx();
 void ek_set_error(const std::string &msg);
 void ek_cuda_check_impl(cudaError_t err, const char *file, int line);
 #define ek_cuda_check(x) ek_cuda_check_impl((x), __FILE__, __LINE__)
+
+/* DLPack releases (ek_dlpack.cpp).  ek_dlpack_pending counts queued releases: exported tensors dropped on any thread
+   and freed imports whose producer has not been told yet.  Entry points call ek_dlpack_drain(), one atomic load when
+   nothing is queued; `wait` (ek_sync, ek_shutdown) waits for every freed import's last use and releases it. */
+extern std::atomic<uint32_t> ek_dlpack_pending;
+void ek_dlpack_drain_slow(bool wait);
+static inline void ek_dlpack_drain(bool wait = false) {
+    if (ek_dlpack_pending.load(std::memory_order_acquire)) ek_dlpack_drain_slow(wait);
+}
+/* queue the release of a freed variable's imported tensor (called by var_free on the owning thread) */
+void ek_dlpack_release_import(EkVariable &v);
+/* ek_shutdown: wait for and release every queued tensor; exports still held by consumers are forgotten */
+void ek_dlpack_shutdown();
+/* the device ek_init() runs on, or will pick */
+int ek_planned_device();
 
 /* kernels (defined in .cu files) */
 /* trig: the body contains an operation of the extension instantiations (ek_isa.h ek_dop_ext: tan ... carlson_rc) */

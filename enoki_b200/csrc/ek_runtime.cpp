@@ -30,6 +30,15 @@ EkContext &ek_ctx() {
 
 void ek_set_error(const std::string &msg) { g_error = msg; }
 
+int ek_planned_device() {
+    if (g_ctx && g_ctx->initialized) return g_ctx->device;
+    if (g_device_request >= 0) return g_device_request;
+    const char *lr = getenv("LOCAL_RANK");
+    if (!lr) return 0;
+    int n = ek_device_count();
+    return n ? atoi(lr) % n : atoi(lr);
+}
+
 void ek_cuda_check_impl(cudaError_t err, const char *file, int line) {
     if (err != cudaSuccess) {
         /* common.cu:268-286: CUDA failures are fatal */
@@ -83,11 +92,7 @@ int ek_init(void) {
         ek_set_error("ek_init(): no CUDA device available -- this backend has no CPU fallback");
         return -1;
     }
-    ctx.device = g_device_request >= 0 ? g_device_request : 0;
-    if (g_device_request < 0) {
-        const char *lr = getenv("LOCAL_RANK");
-        if (lr) ctx.device = atoi(lr) % n;
-    }
+    ctx.device = ek_planned_device();
     ek_cuda_check(cudaSetDevice(ctx.device));
     cudaDeviceProp prop;
     ek_cuda_check(cudaGetDeviceProperties(&prop, ctx.device));
@@ -114,6 +119,7 @@ int ek_fast_mode(void) { return ek_ctx().fast_mode; }
 void ek_shutdown(void) {
     if (!g_ctx) return;
     EkContext &ctx = *g_ctx;
+    ek_dlpack_shutdown();
     if (ctx.initialized) {
         cudaStreamSynchronize(ctx.stream);
         for (auto &v : ctx.vars) {
@@ -128,6 +134,7 @@ void ek_shutdown(void) {
         if (ctx.flush_buf) cudaFree(ctx.flush_buf);
         cudaEventDestroy(ctx.ev_start); cudaEventDestroy(ctx.ev_stop);
         cudaEventDestroy(ctx.tm_start); cudaEventDestroy(ctx.tm_stop);
+        if (ctx.handoff_event) cudaEventDestroy(ctx.handoff_event);
         cudaStreamDestroy(ctx.stream);
     }
     delete g_ctx;
@@ -135,6 +142,11 @@ void ek_shutdown(void) {
 }
 
 /* ------------------------------------------------------------------ allocator */
+static void sync_streams() {
+    ek_cuda_check(cudaStreamSynchronize(g_ctx->stream));
+    if (g_ctx->d2h_stream) ek_cuda_check(cudaStreamSynchronize(g_ctx->d2h_stream));
+}
+
 static void *alloc_impl(int kind, size_t size) {
     EkContext &ctx = ek_ctx();
     if (ek_init() != 0) { fprintf(stderr, "enoki_b200: %s\n", ek_last_error()); exit(EXIT_FAILURE); }
@@ -158,7 +170,7 @@ static void *alloc_impl(int kind, size_t size) {
         if (err == cudaErrorMemoryAllocation) {       /* jit.cu:1715-1723: sync, trim, retry once */
             cudaGetLastError();
             if (ctx.pre_trim_hook) ctx.pre_trim_hook(ctx.pre_trim_arg);
-            ek_sync(); ek_malloc_trim();
+            sync_streams(); ek_malloc_trim();   /* (no DLPack drain: this may run inside ek_eval) */
             err = do_alloc();
         }
         ek_cuda_check(err);
@@ -253,9 +265,9 @@ void ek_memcpy_from_device_overlapped(void *dst, const void *src, size_t size) {
 }
 
 void ek_sync(void) {
-    if (!g_ctx || !g_ctx->initialized) return;
-    ek_cuda_check(cudaStreamSynchronize(g_ctx->stream));
-    if (g_ctx->d2h_stream) ek_cuda_check(cudaStreamSynchronize(g_ctx->d2h_stream));
+    if (!g_ctx) return;
+    if (g_ctx->initialized) sync_streams();
+    ek_dlpack_drain(true);
 }
 
 void ek_fill(void *ptr, size_t elem_size, uint64_t value, size_t n) {
@@ -361,6 +373,7 @@ static void var_free(uint32_t first) {
             if (dv.ref_ext == 0 && dv.ref_int == 0) work.push_back(v.extra_dep);
         }
         if (v.data && v.free_data && !v.direct_pointer) ek_free(v.data);
+        if (v.dlpack) ek_dlpack_release_import(v);
         delete v.label; delete v.fmt;
         v = EkVariable();
         ctx.free_handles.push_back(idx);
@@ -446,6 +459,7 @@ int ek_make_managed(uint32_t index) {
     void *p = ek_managed_malloc(bytes);
     ek_cuda_check(cudaMemcpyAsync(p, v->data, bytes, cudaMemcpyDeviceToDevice, ek_ctx().stream));
     if (v->free_data) ek_free(v->data);
+    if (v->dlpack) ek_dlpack_release_import(*v);
     v->data = p; v->free_data = true;
     return 0;
 }
@@ -473,6 +487,7 @@ static int op_arity(ek_op op) {
 }
 
 uint32_t ek_trace_append(ek_type type, ek_op op, uint32_t a, uint32_t b, uint32_t c, uint64_t imm) {
+    ek_dlpack_drain();
     EkContext &ctx = ek_ctx();
     int arity = op_arity(op);
     if (arity < 0 || ek_type_size(type) == 0) { ek_set_error("ek_trace_append(): invalid opcode/type"); return 0; }

@@ -26,6 +26,7 @@
 
 #include <enoki/array.h>
 #include <enoki_b200.h>
+#include <enoki_b200_dlpack.h>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -410,6 +411,25 @@ struct CUDAArray : ArrayBase<value_t<Value>, CUDAArray<Value>> {
     CUDAArray &managed() { cuda_make_managed(m_index); return *this; }
     const CUDAArray &managed() const { cuda_make_managed(m_index); return *this; }
 
+    // ---- DLPack (no counterpart in the reference): zero-copy exchange with libtorch (at::toDLPack / at::fromDLPack)
+    //      and anything else that speaks DLPack; the rules are those of ek_dlpack_export / ek_dlpack_import
+    /// A managed tensor aliasing this array (evaluated first).  `consumer_stream` is the cudaStream_t the consumer uses
+    /// it on (nullptr: none); order that stream after the backend's work with ek_stream_signal_external().
+    DLManagedTensor *to_dlpack(void *consumer_stream = nullptr) const {
+        void *m = ek_dlpack_export(m_index, 0, consumer_stream);
+        if (!m) detail::ek_throw();
+        return (DLManagedTensor *) m;
+    }
+    DLManagedTensorVersioned *to_dlpack_versioned(void *consumer_stream = nullptr) const {
+        void *m = ek_dlpack_export(m_index, 1, consumer_stream);
+        if (!m) detail::ek_throw();
+        return (DLManagedTensorVersioned *) m;
+    }
+    /// An array aliasing `t`, which it owns from here on: the deleter runs once the backend's last use of the buffer
+    /// has completed.  A refused tensor (device, dtype other than this array's, layout, size) stays the caller's.
+    static CUDAArray from_dlpack(DLManagedTensor *t) { return from_dlpack_(t, t ? &t->dl_tensor : nullptr, 0); }
+    static CUDAArray from_dlpack(DLManagedTensorVersioned *t) { return from_dlpack_(t, t ? &t->dl_tensor : nullptr, 1); }
+
     template <size_t Stride, typename Index, typename Mask>
     static CUDAArray gather_(const void *ptr_, const Index &index, const Mask &mask) {
         uint32_t ptr = cuda_var_register_ptr(ptr_);
@@ -459,6 +479,15 @@ struct CUDAArray : ArrayBase<value_t<Value>, CUDAArray<Value>> {
         cuda_host_free(instances); cuda_host_free(sizes); free(lists);
         m_cached_partition = groups;
         return *groups;
+    }
+
+    static CUDAArray from_dlpack_(void *managed, const DLTensor *t, int versioned) {
+        const int k = (int) Type;          /* EnokiType: Int8 = 1, UInt8, Int16, ..., UInt64 = 8, Float16 .. Float64, Bool */
+        const uint8_t code = k <= 8 ? (k % 2 ? kDLInt : kDLUInt) : Type == EnokiType::Bool ? kDLBool : kDLFloat;
+        if (t && (t->dtype.code != code || t->dtype.bits != 8 * sizeof(Value)))
+            throw std::runtime_error("CUDAArray::from_dlpack(): the tensor's dtype (code " + std::to_string(t->dtype.code) +
+                                     ", " + std::to_string(t->dtype.bits) + " bits) is not this array's");
+        return from_index_(detail::ek_chk(ek_dlpack_import(managed, versioned)));
     }
 
     Index index_() const { return m_index; }

@@ -235,6 +235,35 @@ EK_API void  ek_memcpy_from_device_overlapped(void *dst, const void *src, size_t
 /* extension: device-to-device copy on the runtime's stream (PyTorch / CuPy interop, src/python/common.h:1085-1215) */
 EK_API void  ek_memcpy_device_async(void *dst, const void *src, size_t size);
 
+/* ------------------------------------------------------------------ DLPack (no counterpart in the reference)
+ * Zero-copy exchange of device buffers with other frameworks (torch, CuPy, JAX).  The structures are in
+ * enoki_b200_dlpack.h.  `versioned` selects DLManagedTensorVersioned (1) or the legacy DLManagedTensor (0).
+ *
+ * Export: evaluates the variable, takes an external reference on it and returns a managed tensor aliasing its buffer
+ *   (kDLCUDA on ek_device(), 1-D shape {size}, strides NULL, byte_offset 0).  Float16/32/64 <-> kDLFloat, Int8..64 <->
+ *   kDLInt, UInt8..64 <-> kDLUInt, Mask <-> kDLBool 8; pointer arrays are refused.  `consumer_stream` (a
+ *   cudaStream_t, or NULL when the consumer declared none) is the stream the consumer uses the buffer on.  The
+ *   tensor's deleter may run on any thread: it makes no runtime call, records an event on the consumer stream and
+ *   queues the release; the owning thread makes the backend's stream wait on that event and drops the reference at
+ *   its next entry into the runtime (ek_eval, ek_sync, ek_trace_append, ek_dlpack_*, ek_shutdown).
+ * Import: returns a variable (reference count 1) that aliases the tensor and owns it.  Only kDLCUDA memory on
+ *   ek_device(), lanes 1, the dtypes above and C-contiguous data (strides NULL or compact row-major, any ndim, any
+ *   byte_offset aligned to the element) of 1 .. 2^32-1 elements are accepted; a versioned tensor must be of major
+ *   version 1 and writable.  A refused tensor stays the caller's, and ek_last_error() names the reason; the checks
+ *   make no CUDA call.  When the variable is freed, an event is recorded on the backend's stream and the producer's
+ *   deleter is called once that event has completed (polled at later entries; ek_sync and ek_shutdown wait for it).
+ *   The buffer never reaches the allocator: ek_free, its free lists and ek_malloc_trim never see it. */
+EK_API void    *ek_dlpack_export(uint32_t index, int versioned, void *consumer_stream);
+EK_API uint32_t ek_dlpack_import(void *managed, int versioned);
+/* the CUDA device the backend runs on (the one ek_init() picks, before it has run) */
+EK_API int      ek_device(void);
+/* stream hand-off with a foreign cudaStream_t, one event record + stream wait each, no host synchronisation:
+   ek_stream_wait_external: later work of the backend waits for what `stream` has enqueued so far;
+   ek_stream_signal_external: later work on `stream` waits for what the backend has enqueued so far.
+   Both initialise the backend; they return 0, or -1 when it cannot be (ek_last_error()). */
+EK_API int      ek_stream_wait_external(void *stream);
+EK_API int      ek_stream_signal_external(void *stream);
+
 /* ------------------------------------------------------------------ reverse-mode tape
  * One tape per value type (Float32 / Float64) like the reference's static
  * Tape<CUDAArray<float>> / Tape<CUDAArray<double>> (autodiff.cpp:207-212,1235-1240).
